@@ -4,6 +4,7 @@ T=50; scans sharded one per GPU).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference ...                     # CPU restatement of the reference path (oracle port)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/<name>.npy
 
 A "step" is one denoising step of the sampling loop (voxelise + kernel maps, conditional +
 unconditional MinkUNetDiff passes, guidance, DPM-Solver++ update, re-quantise) on one 180 000-point
@@ -56,7 +57,7 @@ def measured_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return dict(hbm_gbs=p["hbm_gbs"], tf=p.get("bf16_tflops_sustained", p["bf16_tflops"]), src="of measured (MEASURED_PEAKS.json, sustained)")
-    return dict(hbm_gbs=6650.0, tf=1400.0, src="of fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, tf=989.0, src="of the H100 SXM data sheet (dense FP16 tensor, HBM3; 700 W card, not a measured ceiling)")
 
 
 class ClockSampler:
@@ -127,16 +128,6 @@ def sampled_steps(K: int, T: int):
     return sorted({int(round(j * (T - 1) / max(K - 1, 1))) for j in range(K)}) if K > 1 else [0]
 
 
-def csrc_digest():
-    import hashlib
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "lidiff_b200", "csrc")
-    for f in sorted(os.listdir(d)):
-        if f.endswith((".cu", ".cuh")):
-            h.update(open(os.path.join(d, f), "rb").read())
-    return h.hexdigest()[:16]
-
-
 def run_ours(args, rank, world, local_rank):
     import torch.distributed as dist
     from lidiff_b200.sharding import max_over_ranks
@@ -200,6 +191,8 @@ def run_ours(args, rank, world, local_rank):
         barrier()
         if args.profiler_range:
             torch.cuda.profiler.stop()
+    # what the last timed step handed back: the new noisy points x_t and the x0 prediction the next step's second-order update uses
+    dumped = {"x_t": st["xa"].float().cpu().numpy(), "x0_pred": st["x0s"].double().cpu().numpy()} if args.dump_outputs else None
     launches = eng.launches() - l0
     ms = e0.elapsed_time(e1)
     log(f"timed region: {K} steps in {ms:.1f} ms")
@@ -291,7 +284,6 @@ def run_ours(args, rank, world, local_rank):
     peaks = measured_peaks()
     nconv = len(layers)
     geo = eng.geom
-    pair_opt = int(h.get_option(0))                      # LB2_OPT_TC_PAIR: which Cout classes run on the CTA-pair kernel
     cls_of = lambda e: ("ffma" if not e["tc"] else ("cout256" if e["cout"] == 256 else ("cout128" if e["cout"] == 128 else "cout_le96")))
     acc = {c: dict(flops=0.0, bytes_gs=0.0, bytes_min=0.0, ms=0.0, n=0) for c in ("cout256", "cout128", "cout_le96", "ffma")}
     lvl_of_dm = {d.data_ptr(): l for l, d in enumerate(geo.d_n)}
@@ -316,18 +308,12 @@ def run_ours(args, rank, world, local_rank):
     tot = {k: sum(c[k] for c in acc.values()) for k in ("flops", "bytes_gs", "bytes_min", "n")}
     dom = max(acc, key=lambda k: acc[k]["ms"])
     d = acc[dom]
-    names = {"cout256": ("k_spconv_tc_pair<256> (CTA-pair cta_group::2 sparse conv" if pair_opt >= 1 else "k_spconv_tc_n256 (sparse conv") + ", Cout 256: levels 3-4 + decoder level 3)",
-             "cout128": ("k_spconv_tc_pair<128> (CTA-pair cta_group::2 sparse conv" if pair_opt >= 2 else "k_spconv_tc_small<4> (sparse conv") + ", Cout 128: level-3 encoder, level-2 decoder)",
-             "cout_le96": "k_spconv_tc_small<1-3> (sparse conv, Cout 32 / 64 / 96: levels 0-2)", "ffma": "k_spconv_ffma (Cin=3 stem)"}
-    traffic = traffic_src = None
-    tpath = os.path.join(ROOT, "profiles", "r02_conv_dram_traffic.json")
-    if os.path.exists(tpath):                         # ncu dram bytes per launch: only valid for the kernel sources it was captured on
-        tj = json.load(open(tpath))
-        if tj.get("csrc_digest") == csrc_digest():
-            traffic, traffic_src = tj.get("traffic_bytes_per_launch", {}).get(dom), "profiles/r02_conv_dram_traffic.json (ncu --set full, same kernel sources)"
+    names = {"cout256": "k_spconv_tc<128> (wgmma sparse conv, two CTAs of 128 channels per tile, Cout 256: levels 3-4 + decoder level 3)",
+             "cout128": "k_spconv_tc<128> (wgmma sparse conv, Cout 128: level-3 encoder, level-2 decoder)",
+             "cout_le96": "k_spconv_tc<32 / 64 / 96> (wgmma sparse conv, Cout 32 / 64 / 96: levels 0-2)", "ffma": "k_spconv_ffma (Cin=3 stem)"}
     ach = d["flops"] / max(d["ms"], 1e-9) / 1e9          # FLOP / ms / 1e9 = TFLOP/s
     roofline = {"kernel": names[dom], "bound": "tensor", "achieved": round(ach, 2), "peak": peaks["tf"], "unit": "TFLOP/s",
-                "frac": round(ach / peaks["tf"], 4), "traffic": traffic, "traffic_source": traffic_src, "peak_source": peaks["src"],
+                "frac": round(ach / peaks["tf"], 4), "peak_source": peaks["src"],
                 "algorithmic_flops_per_launch": d["flops"] / max(d["n"], 1), "avg_launch_ms": round(d["ms"] / max(d["n"], 1), 4), "launches": d["n"],
                 "share_of_step": round(d["ms"] / ms_instr, 3),
                 "note": "algorithmic FLOPs = 2*pairs*Cin*Cout per pass (SURVEY 8d); the FP16x3 operand split issues 3 MMAs per product, so "
@@ -351,7 +337,7 @@ def run_ours(args, rank, world, local_rank):
                       "steps_note": "the full T-step trajectory runs once untimed; the timed region replays the listed schedule positions from the saved "
                                     "loop state (3 device copies per step, inside the timed region), so K < T samples the whole trajectory instead of its first K steps",
                       "weights": "seeded random init with reference parameter names, BN statistics calibrated on the scan",
-                      "l2": "per-step working set (several GB of feature maps and maps) exceeds the 126 MB L2; no explicit flush",
+                      "l2": "per-step working set (several GB of feature maps and maps) exceeds the 50 MB L2; no explicit flush",
                       "level_rows_first_last": [pair_hist[0, 13:18].tolist(), pair_hist[-1, 13:18].tolist()]},
            "clocks": clocks.summary(),
            "e2e": {"value": round(K * world / (ms_e2e * 1e-3), 3), "unit": UNIT, "h2d_bytes_per_step": N_POINTS * 3 * 4,
@@ -359,11 +345,22 @@ def run_ours(args, rank, world, local_rank):
                    "what": "same schedule positions through DenoiseEngine.start/advance with pinned HOST buffers: scan + start uploaded, per-step SDE noise H2D and x_t D2H inside the timed region"},
            "gpu_launches": int(launches), "roofline": roofline, "fixed_geometry": fixed, "scan_e2e": scan_e2e,
            "engine": {"cuda_graphs": bool(eng.use_graphs), "graph_replays": int(eng.graph_replays), "lean_activations": bool(eng.lean),
-                      "tc_pair": int(h.get_option(0))}}
+                      }}
     if world == 1 and not args.no_cpu_baseline:
         log("cpu baseline leg")
         out["cpu_baseline"] = cpu_reference(scan.cpu(), pipe, steps=2, warmup=1)
+    if dumped is not None:
+        out["dumped_outputs"] = dump_outputs(args.dump_outputs, dumped)
     return out
+
+
+def dump_outputs(d, arrays):
+    """writes each array as d/<name>.npy (float32 / float64 as computed; 180000 x 3 each, a few MB in all)"""
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, f"{name}.npy"), np.ascontiguousarray(a))
+    log(f"outputs of the last timed step written to {d}: {', '.join(f'{k} {v.dtype} {v.shape}' for k, v in arrays.items())}")
+    return sorted(arrays)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -385,7 +382,7 @@ def cpu_reference(scan, pipe, steps, warmup):
     scan (1/8 of the points, same point density) while the conditioning scan x_cond stays complete — so the U-Net work and the
     (queries x keys) nearest-neighbour search shrink by 8 and the encoder work does not.  Full-scan time per step is then
     2 t_enc + 8 (t_step - 2 t_enc) with t_enc timed once; steps/s = 1 / that.  (A sector of x_cond as well would make the brute-force
-    matching 64x cheaper and overstate the CPU 3.8x: measured 0.0637 against 0.0167 steps/s on the whole scan, profiles/r02_*.)"""
+    matching 64x cheaper and overstate the CPU rate several times.)"""
     from oracle.pipeline import DiffCompletionOracle
     cores = usable_cpus()
     torch.set_num_threads(cores)
@@ -423,8 +420,7 @@ def cpu_reference(scan, pipe, steps, warmup):
     return {"value": round(1.0 / t_full, 5), "unit": UNIT, "cores": cores, "kind": "port",
             "sample": f"{steps} denoising step(s) after {warmup} untimed of the oracle (fp32 torch-CPU restatement of the ME/KeOps/diffusers path, all host threads): noisy points = a "
                       f"45-degree azimuthal sector ({n_s} of the {N_POINTS} points, same density), conditioning scan complete; {t_step:.2f} s per sampled step, "
-                      f"conditioning encoder {t_enc:.2f} s per pass; full-scan estimate 2 t_enc + {N_POINTS / n_s:.1f} (t_step - 2 t_enc) = {t_full:.1f} s per step "
-                      f"(measured on the whole scan: 59.7 s per step on 16 cores)"}
+                      f"conditioning encoder {t_enc:.2f} s per pass; full-scan estimate 2 t_enc + {N_POINTS / n_s:.1f} (t_step - 2 t_enc) = {t_full:.1f} s per step"}
 
 
 def run_reference(args, rank, world):
@@ -469,6 +465,8 @@ def main():
     ap.add_argument("--profiler-range", action="store_true", help="cudaProfilerStart/Stop around the timed region (for ncu --profile-from-start off)")
     ap.add_argument("--no-scan", action="store_true", help="skip the whole-scan (configs[4]) measurement")
     ap.add_argument("--T", type=int, default=T_STEPS, help="schedule length (1000 = BASELINE configs[3])")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write what the last of them computed (x_t, x0_pred) as DIR/<name>.npy")
     args = ap.parse_args()
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))

@@ -1,5 +1,5 @@
 /*
- * lidiff_b200 — C ABI of the B200-native (sm_100a) implementation of the LiDiff denoising hot path.
+ * lidiff_b200 — C ABI of the H100-native (sm_90a) implementation of the LiDiff denoising hot path.
  *
  * The reference (PRBonn/LiDiff) reaches this path through three un-vendored Python packages, not
  * through a C interface (SURVEY.md 8b):
@@ -45,17 +45,6 @@ const char* lb2_last_error(void* handle);
 int         lb2_version(void);
 /* number of kernels this library has launched through `handle` since creation (bench gpu_launches) */
 int64_t     lb2_launch_count(void* handle);
-/* Kernel-selection options of a handle (development / A-B knobs; every setting computes the same results and is exercised by
- * the GPU tests).  Defaults come from the environment variable of the same name (LB2_TC_PAIR, ...) at lb2_create. */
-#define LB2_OPT_TC_PAIR       0   /* CTA-pair cta_group::2 conv kernel: 0 off, 1 = Cout 256, 2 = Cout 256 and 128 (default 2) */
-#define LB2_OPT_TC_N256       1   /* single-CTA register-total kernel for Cout 256 (default 1) */
-#define LB2_OPT_TC_SMALL      2   /* two-drain-warpgroup kernel for Cout <= 128 (default 1) */
-#define LB2_OPT_TC_PERSISTENT 3   /* persistent kernels for LB2_ALGO_TC (default 1; 0 = one CTA per tile) */
-#define LB2_OPT_TC_FULL_LAG   4   /* generic persistent kernel: S-1 gather lookahead (default 0) */
-#define LB2_OPT_TC_NSPLIT     5   /* per-tile kernel: split Cout 256 over two CTAs (default 0) */
-#define LB2_OPT_COUNT         6
-int         lb2_set_option(void* handle, int option, int value);
-int         lb2_get_option(void* handle, int option);   /* value, or a negative LB2_ERR_* */
 /* synchronising read-and-clear of the device status word; bit0 = a coordinate fell outside the key
  * range (10 bit batch, 18 bit signed axes) and was clamped.  Returns the word (>= 0) or an error. */
 int         lb2_read_status(void* handle, void* stream);
@@ -90,9 +79,11 @@ int lb2_unique_build(void* h, void* stream,
                      int32_t* out_coords, int32_t* inverse, int32_t* d_nout, void* scratch);
 
 /* UNWEIGHTED_AVERAGE voxel features (ME.SparseTensorQuantizationMode, pipeline:77): mean of member
- * point features.  `counts` int32[m_cap] scratch. out (m_cap, c). */
+ * point features, out (m_cap, c).  The sums are exact fixed-point sums (2^-61 of the largest member magnitude), so the result
+ * does not depend on the order of the points.  `scratch` >= lb2_voxel_mean_scratch_bytes(m_cap, c) bytes. */
+size_t lb2_voxel_mean_scratch_bytes(int32_t m_cap, int32_t c);
 int lb2_voxel_mean(void* h, void* stream, const float* feats, const int32_t* inverse, int32_t n,
-                   int32_t c, const int32_t* d_m, int32_t m_cap, float* out, int32_t* counts);
+                   int32_t c, const int32_t* d_m, int32_t m_cap, float* out, void* scratch);
 
 /* Kernel map (ME kernel maps for MinkowskiConvolution / ConvolutionTranspose; minkunet.py:17-24,36-42).
  * Output-stationary neighbour table: nbr[k * nbr_stride + o] = input row at coords(o) + offset_k, or -1.
@@ -123,8 +114,8 @@ int lb2_row_order(void* h, void* stream, const uint32_t* row_mask, const int32_t
 
 /* Cost order of the tiles of a map (scheduling only; results do not depend on it): order128[i] / order256[i] = index of the i-th most
  * expensive 128-row tile / 256-row super-tile of the row order `row_perm`, cost = number of kernel offsets the tile has to run (popcount of
- * the OR of its rows' masks); entries beyond the live tile count are -1.  The persistent convolution kernels deal tiles to their CTAs in
- * snake order over this sequence (lb2_conv_desc.tile_order128 / tile_order256), which balances a static assignment to within 1-3 %.
+ * the OR of its rows' masks); entries beyond the live tile count are -1.  A persistent convolution kernel can deal tiles to its CTAs in
+ * snake order over this sequence (lb2_conv_desc.tile_order128 / tile_order256); the one-CTA-per-tile kernel of this build ignores it.
  * order128: cdiv(n_cap,128) ints, order256: cdiv(n_cap,256) ints, scratch: cdiv(n_cap,128) * 4 bytes. */
 int lb2_tile_order(void* h, void* stream, const uint32_t* row_mask, const int32_t* row_perm, const int32_t* d_n, int32_t n_cap,
                    int32_t* order128, int32_t* order256, void* scratch);
@@ -180,8 +171,8 @@ typedef struct {
 
 #define LB2_ALGO_AUTO  0
 #define LB2_ALGO_FFMA  1    /* fp32 CUDA-core implicit GEMM */
-#define LB2_ALGO_TC    2    /* tcgen05 FP16x3 split-precision implicit GEMM (needs weight_packed), persistent CTAs */
-#define LB2_ALGO_TC_TILE 3  /* same math, one CTA per 128-row tile (non-persistent reference variant) */
+#define LB2_ALGO_TC    2    /* wgmma FP16x3 split-precision implicit GEMM (needs weight_packed), one CTA per 128-row tile */
+#define LB2_ALGO_TC_TILE 3  /* the same kernel (kept as an alias: callers that name the per-tile form) */
 int lb2_spconv_forward(void* h, void* stream, const lb2_conv_desc* d, int algo);
 
 /* The same convolution in gather-GEMM-scatter form (what ME's GPU backend does per kernel offset) for levels
@@ -213,7 +204,7 @@ int lb2_pair_list(void* h, void* stream, const int32_t* nbr, int64_t nbr_stride,
 int lb2_spconv_scatter_supported(int32_t c1, int32_t c2, int32_t cout, int32_t kvol);
 int lb2_spconv_scatter(void* h, void* stream, const lb2_scatter_desc* d);
 
-/* FP16 hi/lo split (power-of-two pre-scaled) + UMMA shared-memory image of a (kvol, cin, cout) fp32 weight
+/* FP16 hi/lo split (power-of-two pre-scaled) + wgmma shared-memory image of a (kvol, cin, cout) fp32 weight
  * for LB2_ALGO_TC. */
 size_t lb2_packed_weight_bytes(int32_t kvol, int32_t cin, int32_t cout);
 int lb2_pack_weights(void* h, void* stream, const float* weight, int32_t kvol, int32_t cin, int32_t cout,

@@ -1,7 +1,7 @@
-"""ctypes binding of include/lidiff_b200.h (the C-ABI CUDA library, sm_100a).
+"""ctypes binding of include/lidiff_b200.h (the C-ABI CUDA library, sm_90a).
 
 There is deliberately NO CPU fallback: importing works anywhere (so host logic can be tested), but
-`get_lib()` raises if the shared object is missing and `Lib.handle(device)` raises if no B200 is
+`get_lib()` raises if the shared object is missing and `Lib.handle(device)` raises if no H100 (sm_90) is
 visible.  torch is used only for device memory and streams.
 """
 from __future__ import annotations
@@ -15,7 +15,6 @@ import torch
 _SO = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_C", "liblidiff_b200.so")
 
 ALGO_AUTO, ALGO_FFMA, ALGO_TC, ALGO_TC_TILE = 0, 1, 2, 3
-OPT_TC_PAIR, OPT_TC_N256, OPT_TC_SMALL, OPT_TC_PERSISTENT, OPT_TC_FULL_LAG, OPT_TC_NSPLIT = range(6)
 
 
 class Grid(C.Structure):
@@ -58,8 +57,8 @@ class DpmCoef(C.Structure):
 
 EXPORTS = [
     "lb2_create", "lb2_destroy", "lb2_last_error", "lb2_version", "lb2_launch_count", "lb2_read_status",
-    "lb2_set_option", "lb2_get_option", "lb2_tile_order",
-    "lb2_quantize", "lb2_unique_scratch_bytes", "lb2_unique_build", "lb2_voxel_mean", "lb2_kernel_map",
+    "lb2_tile_order",
+    "lb2_quantize", "lb2_unique_scratch_bytes", "lb2_unique_build", "lb2_voxel_mean_scratch_bytes", "lb2_voxel_mean", "lb2_kernel_map",
     "lb2_spconv_forward", "lb2_packed_weight_bytes", "lb2_pack_weights", "lb2_nn_match", "lb2_linear",
     "lb2_gate_mul", "lb2_gather_rows", "lb2_head_mlp", "lb2_kernel_map_self", "lb2_guidance_dpm_step", "lb2_farthest_point_sample",
     "lb2_row_order", "lb2_row_order_scratch_bytes", "lb2_nn_match_grid",
@@ -95,10 +94,10 @@ class Lib:
         d.lb2_launch_count.argtypes = [C.c_void_p]
         d.lb2_launch_count.restype = C.c_int64
         d.lb2_read_status.argtypes = [C.c_void_p, C.c_void_p]
-        d.lb2_set_option.argtypes = [C.c_void_p, C.c_int, C.c_int]
-        d.lb2_get_option.argtypes = [C.c_void_p, C.c_int]
         d.lb2_unique_scratch_bytes.argtypes = [C.c_int64]
         d.lb2_unique_scratch_bytes.restype = C.c_size_t
+        d.lb2_voxel_mean_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
+        d.lb2_voxel_mean_scratch_bytes.restype = C.c_size_t
         d.lb2_packed_weight_bytes.argtypes = [C.c_int32] * 3
         d.lb2_packed_weight_bytes.restype = C.c_size_t
         vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
@@ -142,14 +141,14 @@ class Lib:
     def handle(self, device) -> "Handle":
         dev = torch.device(device)
         if dev.type != "cuda":
-            raise RuntimeError("lidiff_b200 runs on CUDA (B200, sm_100a) only; no CPU fallback")
+            raise RuntimeError("lidiff_b200 runs on CUDA (H100, sm_90a) only; no CPU fallback")
         idx = dev.index if dev.index is not None else torch.cuda.current_device()
         with self._lock:
             if idx not in self._handles:
                 hp = C.c_void_p()
                 rc = self.dll.lb2_create(idx, C.byref(hp))
                 if rc != 0:
-                    raise RuntimeError(f"lb2_create(device={idx}) failed with {rc} (needs an sm_100 GPU)")
+                    raise RuntimeError(f"lb2_create(device={idx}) failed with {rc} (needs an sm_90 GPU)")
                 self._handles[idx] = Handle(self, hp, idx)
             return self._handles[idx]
 
@@ -174,12 +173,6 @@ class Handle:
     def read_status(self) -> int:
         return int(self.dll.lb2_read_status(self.hp, self._stream()))
 
-    def set_option(self, option: int, value: int):
-        self._check(self.dll.lb2_set_option(self.hp, int(option), int(value)), "set_option")
-
-    def get_option(self, option: int) -> int:
-        return int(self.dll.lb2_get_option(self.hp, int(option)))
-
     # -- coordinate manager ------------------------------------------------------------------------
     def new_grid(self, n_cap: int):
         cap = 1 << max(4, (2 * n_cap - 1).bit_length())
@@ -202,9 +195,13 @@ class Handle:
         self._check(self.dll.lb2_unique_build(self.hp, self._stream(), _ptr(in_f), _ptr(in_i), _ptr(d_nin), int(n_cap), int(ts_floor),
                                               self._grid(grid), _ptr(out_coords), _ptr(inverse), _ptr(d_nout), _ptr(scratch)), "lb2_unique_build")
 
-    def voxel_mean(self, feats, inverse, n, c, d_m, m_cap, out, counts):
+    def voxel_mean_scratch(self, m_cap: int, c: int) -> torch.Tensor:
+        nbytes = int(self.dll.lb2_voxel_mean_scratch_bytes(int(m_cap), int(c)))
+        return torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+
+    def voxel_mean(self, feats, inverse, n, c, d_m, m_cap, out, scratch):
         self._check(self.dll.lb2_voxel_mean(self.hp, self._stream(), _ptr(feats), _ptr(inverse), int(n), int(c), _ptr(d_m), int(m_cap),
-                                            _ptr(out), _ptr(counts)), "lb2_voxel_mean")
+                                            _ptr(out), _ptr(scratch)), "lb2_voxel_mean")
 
     def kernel_map(self, grid_in, out_coords, d_nout, nout_cap, ks, step, nbr, nbr_stride, pair_count=None, row_mask=None):
         self._check(self.dll.lb2_kernel_map(self.hp, self._stream(), self._grid(grid_in), _ptr(out_coords), _ptr(d_nout), int(nout_cap),

@@ -1,8 +1,8 @@
-// Dispatch of lb2_spconv_forward to the CUDA-core (spconv_ffma.cu) or tcgen05 (spconv_tc.cu) variant.
+// Dispatch of lb2_spconv_forward to the CUDA-core (spconv_ffma.cu) or wgmma (spconv_tc.cu) variant.
 #include "common.cuh"
 
 int lb2_spconv_ffma_launch(Lb2Handle* h, cudaStream_t s, const lb2_conv_desc* d);
-int lb2_spconv_tc_launch(Lb2Handle* h, cudaStream_t s, const lb2_conv_desc* d, bool persistent);
+int lb2_spconv_tc_launch(Lb2Handle* h, cudaStream_t s, const lb2_conv_desc* d);
 bool lb2_spconv_tc_supported(const lb2_conv_desc* d);
 
 extern "C" int lb2_spconv_forward(void* handle, void* stream, const lb2_conv_desc* d, int algo) {
@@ -29,9 +29,9 @@ extern "C" int lb2_spconv_forward(void* handle, void* stream, const lb2_conv_des
     if (algo == LB2_ALGO_TC || algo == LB2_ALGO_TC_TILE) {
         if (!d->weight_packed || !lb2_spconv_tc_supported(d))
             return lb2_fail(h, LB2_ERR_UNSUP, "tensor-core variant does not support this layer%s", "");
-        return lb2_spconv_tc_launch(h, s, d, algo == LB2_ALGO_TC);
+        return lb2_spconv_tc_launch(h, s, d);
     }
-    if (algo == LB2_ALGO_AUTO && d->weight_packed && lb2_spconv_tc_supported(d)) return lb2_spconv_tc_launch(h, s, d, true);
+    if (algo == LB2_ALGO_AUTO && d->weight_packed && lb2_spconv_tc_supported(d)) return lb2_spconv_tc_launch(h, s, d);
     if (!have_f32) return lb2_fail(h, LB2_ERR_UNSUP, "companion-only inputs need a tensor-core variant that takes this layer%s", "");
     return lb2_spconv_ffma_launch(h, s, d);
 }

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the lidiff_b200 CUDA library (sm_100a only).
+// Shared device/host helpers for the lidiff_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,13 +11,13 @@ struct Lb2Handle {
     int      num_sms;
     int64_t  launches;
     int32_t* d_status;      // device status word (bit0: coordinate out of key range)
-    int      opt[LB2_OPT_COUNT];   // kernel-selection options (lb2_set_option)
     uint32_t configured;    // bit per kernel whose max-dynamic-shared-memory attribute has been set on this handle's device
     char     err[512];
 };
 
 // kernels that need more than 48 KB of dynamic shared memory: the attribute is per-device state, the handle is per device
-enum { LB2_K_TC = 0, LB2_K_TC2, LB2_K_TC3, LB2_K_TC4, LB2_K_TC5_256, LB2_K_TC5_128, LB2_K_SCATTER, LB2_K_NN_TABLE };
+// (LB2_K_TC and LB2_K_SCATTER: one bit per instantiation, N = 32, 64, 96, 128)
+enum { LB2_K_TC = 0, LB2_K_SCATTER = 4, LB2_K_NN_TABLE = 8 };
 template <class K>
 static inline cudaError_t lb2_configure_smem(Lb2Handle* h, int bit, K kernel, int bytes) {
     if (h->configured & (1u << bit)) return cudaSuccess;

@@ -22,19 +22,9 @@ extern "C" int lb2_create(int device, void** handle) {
     if (cudaSetDevice(device) != cudaSuccess) return LB2_ERR_CUDA;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return LB2_ERR_CUDA;
-    if (prop.major != 10) return LB2_ERR_UNSUP;          // sm_100a binary only
+    if (prop.major != 9) return LB2_ERR_UNSUP;           // sm_90a binary only
     Lb2Handle* h = new Lb2Handle();
     h->device = device; h->num_sms = prop.multiProcessorCount; h->launches = 0; h->err[0] = 0; h->configured = 0;
-    {
-        auto env = [](const char* name, int dflt) { const char* e = getenv(name); return (e && e[0]) ? atoi(e) : dflt; };
-        h->opt[LB2_OPT_TC_PAIR] = env("LB2_TC_PAIR", 2);
-        h->opt[LB2_OPT_TC_N256] = env("LB2_TC_N256", 1);
-        h->opt[LB2_OPT_TC_SMALL] = env("LB2_TC_SMALL", 1);
-        h->opt[LB2_OPT_TC_PERSISTENT] = env("LB2_TC_PERSISTENT", 1);
-        const char* lag = getenv("LB2_TC_LAG");
-        h->opt[LB2_OPT_TC_FULL_LAG] = (lag && lag[0] == 'f') ? 1 : 0;
-        h->opt[LB2_OPT_TC_NSPLIT] = env("LB2_TC_NSPLIT", 0);
-    }
     if (cudaMalloc(&h->d_status, sizeof(int32_t)) != cudaSuccess) { delete h; return LB2_ERR_CUDA; }
     cudaMemset(h->d_status, 0, sizeof(int32_t));
     *handle = h;
@@ -46,19 +36,6 @@ extern "C" void lb2_destroy(void* handle) {
     if (!h) return;
     cudaFree(h->d_status);
     delete h;
-}
-
-extern "C" int lb2_set_option(void* handle, int option, int value) {
-    Lb2Handle* h = (Lb2Handle*)handle;
-    LB2_REQUIRE(h, h && option >= 0 && option < LB2_OPT_COUNT, "set_option");
-    h->opt[option] = value;
-    return LB2_OK;
-}
-
-extern "C" int lb2_get_option(void* handle, int option) {
-    Lb2Handle* h = (Lb2Handle*)handle;
-    if (!h || option < 0 || option >= LB2_OPT_COUNT) return LB2_ERR_ARG;
-    return h->opt[option];
 }
 
 extern "C" const char* lb2_last_error(void* handle) {
@@ -290,35 +267,71 @@ extern "C" int lb2_unique_build(void* handle, void* stream, const float* in_f, c
 // ---------------------------------------------------------------------------------------------------
 // voxel mean features
 // ---------------------------------------------------------------------------------------------------
-__global__ void k_voxel_accum(const float* __restrict__ feats, const int* __restrict__ inverse, int n, int c,
-                              float* __restrict__ out, int* __restrict__ counts) {
+// The sums are exact and independent of the order in which points arrive: each (voxel, channel) sum is accumulated in int64 fixed point
+// at a scale set by the largest member magnitude and the member count (every value v becomes round(v * 2^s) with |sum| < 2^61), then
+// divided by the count in fp64 and rounded once to fp32.  fp32 atomics would make the last bits, and through the re-voxelisation of the
+// next steps whole trajectories, differ from run to run.
+__device__ __forceinline__ int voxel_fix_shift(float maxabs, int count) {
+    int e;
+    frexpf(maxabs, &e);                                   // maxabs < 2^e
+    return 61 - e - (32 - __clz(count));                  // count * 2^(e + s) <= 2^61
+}
+
+__global__ void k_voxel_absmax(const float* __restrict__ feats, const int* __restrict__ inverse, int n, int c,
+                               unsigned* __restrict__ maxabs, int* __restrict__ counts) {
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)n * c) return;
     int i = (int)(t / c), j = (int)(t % c);
     int r = inverse[i];
-    atomicAdd(out + (long long)r * c + j, feats[t]);
+    atomicMax(maxabs + (long long)r * c + j, __float_as_uint(fabsf(feats[t])));      // non-negative floats order like uints
     if (j == 0) atomicAdd(counts + r, 1);
 }
 
-__global__ void k_voxel_div(float* __restrict__ out, const int* __restrict__ counts, const int* __restrict__ d_m,
-                            int m_cap, int c) {
+__global__ void k_voxel_accum(const float* __restrict__ feats, const int* __restrict__ inverse, int n, int c,
+                              const float* __restrict__ maxabs, const int* __restrict__ counts, unsigned long long* __restrict__ sums) {
+    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)n * c) return;
+    int i = (int)(t / c), j = (int)(t % c);
+    int r = inverse[i];
+    const long long e = (long long)r * c + j;
+    const float m = maxabs[e];
+    if (!(m > 0.f) || !isfinite(m)) return;               // all zero (sum 0), or non-finite (k_voxel_div writes NaN)
+    const long long q = llrint(ldexp((double)feats[t], voxel_fix_shift(m, counts[r])));
+    atomicAdd(sums + e, (unsigned long long)q);           // two's complement: the wrapped unsigned sum is the signed sum
+}
+
+__global__ void k_voxel_div(float* __restrict__ out, const int* __restrict__ counts, const unsigned long long* __restrict__ sums,
+                            const int* __restrict__ d_m, int m_cap, int c) {
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     int m = d_m ? min(*d_m, m_cap) : m_cap;
     if (t >= (long long)m * c) return;
-    out[t] = __fdiv_rn(out[t], (float)counts[t / c]);
+    const float mx = out[t];                              // out holds the largest magnitude until here
+    const int cnt = counts[t / c];
+    if (!isfinite(mx)) { out[t] = __int_as_float(0x7fffffff); return; }
+    if (!(mx > 0.f) || cnt == 0) { out[t] = cnt == 0 ? __fdiv_rn(0.f, 0.f) : 0.f; return; }
+    const double sum = ldexp((double)(long long)sums[t], -voxel_fix_shift(mx, cnt));
+    out[t] = __double2float_rn(sum / (double)cnt);
+}
+
+extern "C" size_t lb2_voxel_mean_scratch_bytes(int32_t m_cap, int32_t c) {
+    return (size_t)m_cap * c * sizeof(unsigned long long) + (size_t)m_cap * sizeof(int);
 }
 
 extern "C" int lb2_voxel_mean(void* handle, void* stream, const float* feats, const int32_t* inverse, int32_t n,
-                              int32_t c, const int32_t* d_m, int32_t m_cap, float* out, int32_t* counts) {
+                              int32_t c, const int32_t* d_m, int32_t m_cap, float* out, void* scratch) {
     Lb2Handle* h = (Lb2Handle*)handle;
-    LB2_REQUIRE(h, h && feats && inverse && out && counts && n > 0 && c > 0 && m_cap > 0, "voxel_mean");
+    LB2_REQUIRE(h, h && feats && inverse && out && scratch && n > 0 && c > 0 && m_cap > 0, "voxel_mean");
     cudaStream_t s = (cudaStream_t)stream;
+    unsigned long long* sums = (unsigned long long*)scratch;
+    int* counts = (int*)(sums + (size_t)m_cap * c);
     if (cudaMemsetAsync(out, 0, (size_t)m_cap * c * sizeof(float), s) != cudaSuccess ||
-        cudaMemsetAsync(counts, 0, (size_t)m_cap * sizeof(int), s) != cudaSuccess)
+        cudaMemsetAsync(scratch, 0, lb2_voxel_mean_scratch_bytes(m_cap, c), s) != cudaSuccess)
         return lb2_fail(h, LB2_ERR_CUDA, "voxel_mean memset%s", "");
-    k_voxel_accum<<<cdiv((long long)n * c, 256), 256, 0, s>>>(feats, inverse, n, c, out, counts);
+    k_voxel_absmax<<<cdiv((long long)n * c, 256), 256, 0, s>>>(feats, inverse, n, c, (unsigned*)out, counts);
+    LB2_POST_LAUNCH(h, "k_voxel_absmax");
+    k_voxel_accum<<<cdiv((long long)n * c, 256), 256, 0, s>>>(feats, inverse, n, c, out, counts, sums);
     LB2_POST_LAUNCH(h, "k_voxel_accum");
-    k_voxel_div<<<cdiv((long long)m_cap * c, 256), 256, 0, s>>>(out, counts, d_m, m_cap, c);
+    k_voxel_div<<<cdiv((long long)m_cap * c, 256), 256, 0, s>>>(out, counts, sums, d_m, m_cap, c);
     LB2_POST_LAUNCH(h, "k_voxel_div");
     return LB2_OK;
 }
@@ -488,16 +501,14 @@ extern "C" int lb2_kernel_map_self(void* handle, void* stream, lb2_grid grid, co
 // ---------------------------------------------------------------------------------------------------
 // row order: sort of the output rows by their neighbour mask, so that the 128-row tiles of the convolution
 // kernels are (nearly) homogeneous in which kernel offsets are populated and skip the rest.
-//   kvol <= 8 : one counting-sort pass on the 8-bit mask itself.
+//   kvol <= 8 : one pass of the same stable radix sort on the 8-bit mask itself.
 //   kvol == 27: stable LSD radix sort (3 passes of 9 bits) on the 27-bit key
 //                  [ 2 or more off-centre neighbours ? 1 : 0 | mask without the (always set) centre bit ]
 //               i.e. centre-only rows first, then the rows with exactly one neighbour grouped by it (tiles that need
-//               two offsets), then everything else in mask order.  Measured on the bench trajectory the issued
-//               (tile, offset) slots drop by 10-30 % on the levels with 3-14 neighbours per row against the
-//               previous 55-class bucketing (profiles/r01_row_order_waste.txt).
-// The order inside a group of equal keys is irrelevant for the results (each output row is computed independently).
+//               two offsets), then everything else in mask order.
+// Both sorts are stable, so the order is the same on every run.  It matters for the last bits: the tensor-core convolution
+// groups the kernel offsets a tile runs for its two-level accumulation, and a tile's offsets depend on which rows share it.
 // ---------------------------------------------------------------------------------------------------
-#define RO_BINS 256
 #define RS_BITS 9
 #define RS_BINS (1 << RS_BITS)
 #define RS_CHUNK 2048                       // rows per block and pass
@@ -527,6 +538,7 @@ struct RsSrc {
     const unsigned* keys;        // mode 0: keys[i] (ping-pong buffer of the previous pass)
     const unsigned* mask;        // mode 1: ro_key27(mask[i])            (first pass of a mask-only sort, value = i)
                                  // mode 3: ro_key27(mask[vals_in[i]])   (first mask pass behind the Morton passes)
+                                 // mode 4: mask[i] & 0xff               (the one pass of an 8-bit mask sort, value = i)
     const int4* coords;          // mode 2: ro_morton(coords[i])          (first Morton pass, value = i)
     const int* vals;             // values of the previous pass or NULL (value = i)
     int mode, coord_shift;
@@ -536,6 +548,7 @@ __device__ __forceinline__ unsigned rs_key(const RsSrc& s, int i) {
         case 0: return s.keys[i];
         case 1: return ro_key27(s.mask[i]);
         case 2: return ro_morton(s.coords[i], s.coord_shift);
+        case 4: return s.mask[i] & 0xffu;
         default: return ro_key27(s.mask[s.vals[i]]);
     }
 }
@@ -619,56 +632,10 @@ __global__ void __launch_bounds__(32 * RS_WARPS) k_rs_scatter(const RsSrc src, c
     }
 }
 
-__device__ __forceinline__ int ro_bucket(unsigned mask, int kvol) {
-    (void)kvol;
-    return (int)(mask & 0xffu);
-}
-
-__global__ void k_ro_hist(const unsigned* __restrict__ mask, const int* __restrict__ d_n, int n_cap, int kvol, int* __restrict__ bins) {
-    __shared__ int sh[RO_BINS];
-    for (int i = threadIdx.x; i < RO_BINS; i += blockDim.x) sh[i] = 0;
-    __syncthreads();
-    const int n = d_n ? min(*d_n, n_cap) : n_cap;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) atomicAdd(&sh[ro_bucket(mask[i], kvol)], 1);
-    __syncthreads();
-    for (int i = threadIdx.x; i < RO_BINS; i += blockDim.x) if (sh[i]) atomicAdd(&bins[i], sh[i]);
-}
-
-__global__ void k_ro_scan(int* __restrict__ bins) {        // 1 block of RO_BINS threads: exclusive scan in place
-    __shared__ int sh[RO_BINS];
-    const int t = threadIdx.x;
-    const int v = bins[t];
-    sh[t] = v;
-    __syncthreads();
-    for (int d = 1; d < RO_BINS; d <<= 1) {
-        const int u = (t >= d) ? sh[t - d] : 0;
-        __syncthreads();
-        sh[t] += u;
-        __syncthreads();
-    }
-    bins[t] = sh[t] - v;
-}
-
-__global__ void k_ro_scatter(const unsigned* __restrict__ mask, const int* __restrict__ d_n, int n_cap, int kvol,
-                             int* __restrict__ cursor, int* __restrict__ perm) {
-    __shared__ int cnt[RO_BINS];
-    __shared__ int base[RO_BINS];
-    for (int i = threadIdx.x; i < RO_BINS; i += blockDim.x) cnt[i] = 0;
-    __syncthreads();
-    const int n = d_n ? min(*d_n, n_cap) : n_cap;
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    int b = -1, local = 0;
-    if (i < n) { b = ro_bucket(mask[i], kvol); local = atomicAdd(&cnt[b], 1); }
-    __syncthreads();
-    for (int j = threadIdx.x; j < RO_BINS; j += blockDim.x) if (cnt[j]) base[j] = atomicAdd(&cursor[j], cnt[j]);
-    __syncthreads();
-    if (i < n) perm[base[b] + local] = i;
-}
-
 static int rs_blocks(int n_cap) { return cdiv(n_cap, RS_CHUNK); }
 
 // scratch layout: [nblk][RS_BINS] histogram, [6][RS_BINS] per-pass bin totals, then keys A, keys B, vals A (n_cap each);
-// kvol <= 8 uses the first RO_BINS ints only
+// kvol <= 8 uses the histogram and the first pass total only
 extern "C" size_t lb2_row_order_scratch_bytes(int32_t n_cap) {
     return ((size_t)RS_BINS * (rs_blocks(n_cap) + 6) + 3 * (size_t)n_cap) * sizeof(int);
 }
@@ -710,14 +677,18 @@ extern "C" int lb2_row_order(void* handle, void* stream, const uint32_t* row_mas
         }
         return LB2_OK;
     }
-    int* bins = (int*)scratch;
-    if (cudaMemsetAsync(bins, 0, RO_BINS * sizeof(int), s) != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "row_order memset%s", "");
-    k_ro_hist<<<std::min<unsigned>(cdiv(n_cap, 256), 1024u), 256, 0, s>>>(row_mask, d_n, n_cap, kvol, bins);
-    LB2_POST_LAUNCH(h, "k_ro_hist");
-    k_ro_scan<<<1, RO_BINS, 0, s>>>(bins);
-    LB2_POST_LAUNCH(h, "k_ro_scan");
-    k_ro_scatter<<<cdiv(n_cap, 256), 256, 0, s>>>(row_mask, d_n, n_cap, kvol, bins, perm);
-    LB2_POST_LAUNCH(h, "k_ro_scatter");
+    // kvol <= 8: one pass of the same stable radix sort on the 8-bit mask (rows of equal mask keep their index order, so the
+    // order, and with it the tiles' accumulation grouping, is the same on every run)
+    const int nblk = rs_blocks(n_cap);
+    int* hist = (int*)scratch;
+    int* total = hist + (size_t)RS_BINS * nblk;
+    if (cudaMemsetAsync(total, 0, RS_BINS * sizeof(int), s) != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "row_order memset%s", "");
+    RsSrc src;
+    src.mask = row_mask; src.coords = nullptr; src.coord_shift = 0; src.keys = nullptr; src.vals = nullptr; src.mode = 4;
+    k_rs_hist<<<nblk, 256, 0, s>>>(src, d_n, n_cap, 0, hist, total);
+    LB2_POST_LAUNCH(h, "k_rs_hist");
+    k_rs_scatter<<<nblk, 32 * RS_WARPS, 0, s>>>(src, d_n, n_cap, 0, hist, total, nullptr, perm);
+    LB2_POST_LAUNCH(h, "k_rs_scatter");
     return LB2_OK;
 }
 

@@ -4,18 +4,19 @@
 // (in,out) pairs of a kernel offset are compacted first, so every MMA row is a real pair:
 //
 //   for each offset k (except the centre, which the output-stationary kernel handles as a dense GEMM):
-//       Y[pairs_k, Cout] = X[pair_in] @ W[k]          tcgen05, FP16x3 split, accumulator in TMEM
-//       out[pair_out] += Y                             red.global.add.v4.f32
+//       Y[pairs_k, Cout] = X[pair_in] @ W[k]          wgmma, FP16x3 split, accumulator in registers
+//       out[pair_out] += Y                             red.global.add.v2.f32
 //
 // Persistent, weight-stationary: one CTA per SM walks a contiguous range of 128-pair tiles (sorted by k), so
 // the packed W[k] (all Cin chunks, <= 96 KB) is loaded into shared memory once per run of equal k and every
 // MMA reads B from there; only the gathered A rows stream through the stage ring.
-//   warps 0-3 A producers (gather by pair_in, fp16 hi/lo split, SWIZZLE_128B image)     warp 4 MMA issuer
-//   warp 5 weight loader (cp.async.bulk)     warps 6-9 scatter epilogue (tcgen05.ld -> red.add), ping-pong TMEM
+//   warpgroup 0   A producers (gather by pair_in, fp16 hi/lo split, SWIZZLE_128B image); thread 0 also loads W[k]
+//                 (cp.async.bulk) at the start of every run of equal k
+//   warpgroups 1, 2  consumers: pairs [0, 64) / [64, 128) of the tile, wgmma, then red.add of the rows to out[pair_out]
 // The scattered buffer is the `pre_add` input of the centre convolution, which applies BN/ReLU/residual/gate.
+// (A tile of one offset has at most 3 x 12 chained MMA steps: no two-level accumulation is needed.)
 //
-// Stands behind ME.MinkowskiConvolution forward (ME's own GPU algorithm is this gather-GEMM-scatter),
-// /root/reference/lidiff/models/minkunet.py:17-24,53-66.
+// Stands behind ME.MinkowskiConvolution forward (ME's own GPU algorithm is this gather-GEMM-scatter).
 #include "common.cuh"
 #include <algorithm>
 #include "tc_common.cuh"
@@ -23,11 +24,10 @@
 namespace sc {
 using namespace tc;
 
-constexpr int THREADS = 320;
+constexpr int THREADS = 384;
+constexpr int NUM_CONSUMER_WARPS = 8;
 constexpr int MAX_STAGES = 4;
 constexpr int MAX_KVOL = 27;
-constexpr int SLAB_PITCH = 36;
-constexpr int SLAB_BYTES = BM * SLAB_PITCH * 4;
 
 struct Params {
     int c1, c2, cout, kvol, nchunks, stages, npass;
@@ -41,13 +41,14 @@ struct Params {
     const void* in1_h[2];
     const void* in2_h[2];
     float* out[2];
-    int acc_stride, tmem_cols;
 };
 
+template <int N>
 __global__ void __launch_bounds__(THREADS, 1) k_spconv_scatter(const Params p) {
     extern __shared__ unsigned char smem_raw[];
     __shared__ int s_koff[MAX_KVOL + 1];
     __shared__ int s_toff[MAX_KVOL + 1];
+    __shared__ __align__(8) uint64_t bars[2 * MAX_STAGES + 2];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ctot = p.c1 + p.c2;
     if (threadIdx.x <= p.kvol) { s_koff[threadIdx.x] = p.koff[threadIdx.x]; s_toff[threadIdx.x] = p.tile_off[threadIdx.x]; }
@@ -55,35 +56,22 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_scatter(const Params p) {
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     unsigned char* gen = smem_raw + (base - raw);
-    const uint32_t b_tile = (uint32_t)p.cout * 128u;
+    constexpr uint32_t b_tile = (uint32_t)N * 128u;
     const uint32_t w_bytes = (uint32_t)p.nchunks * 2u * b_tile;          // resident W[k]
     const uint32_t a_stage = 2u * A_TILE;
     unsigned char* a_gen = gen + w_bytes;
     const uint32_t a_base = base + w_bytes;
-    float* slab = reinterpret_cast<float*>(a_gen + (size_t)p.stages * a_stage);         // [4 warps][32][SLAB_PITCH] epilogue transpose
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(slab) + SLAB_BYTES);
-    uint32_t* misc = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 6);
     const uint32_t bar0 = smem_u32(bars);
     auto full_a = [&](int s) { return bar0 + 8u * s; };
     auto empty_a = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
     const uint32_t w_full = bar0 + 8u * (2 * MAX_STAGES), w_empty = bar0 + 8u * (2 * MAX_STAGES + 1);
-    auto acc_full = [&](int b) { return bar0 + 8u * (2 * MAX_STAGES + 2 + b); };
-    auto acc_empty = [&](int b) { return bar0 + 8u * (2 * MAX_STAGES + 4 + b); };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.stages; ++s) { mbar_init(full_a(s), 128); mbar_init(empty_a(s), 1); }
-        mbar_init(w_full, 1); mbar_init(w_empty, 1);
-        for (int b = 0; b < 2; ++b) { mbar_init(acc_full(b), 1); mbar_init(acc_empty(b), 128); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(full_a(s), 128); mbar_init(empty_a(s), NUM_CONSUMER_WARPS); }
+        mbar_init(w_full, 1); mbar_init(w_empty, NUM_CONSUMER_WARPS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&misc[0])), "r"((uint32_t)p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_d = misc[0];
 
     // this CTA's contiguous range of (pass, tile) work items
     const int tiles_per_pass = s_toff[p.kvol];
@@ -101,20 +89,32 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_scatter(const Params p) {
     };
 
     if (warp < 4) {
-        // =========================== A producers ===========================
+        // =========================== producers ===========================
         const int sub = threadIdx.x & 7, rbase = threadIdx.x >> 3;
-        const int D = p.stages - 1;
-        int it = 0, arrived = 0;
-        bool any_h = false;
+        // cp.async lookahead: stages still landing while the next is issued.  S - 2, not S - 1: a consumer releases a stage only once it
+        // holds the next one (wgmma_wait<1>), so the producers must be able to publish stage i + 1 while stage i - 1 is still held
+        const int D = max(p.stages - 2, 0);
+        int it = 0, arrived = 0, wrun = -1, cur_k = -1, cur_pass = -1;
         for (int T = t_begin; T < t_end; ++T) {
             int pass, k, pbase, cnt;
             decode(T, pass, k, pbase, cnt);
+            if (threadIdx.x == 0 && (k != cur_k || pass != cur_pass)) {
+                // new run of equal k: W[k] replaces the previous weights once the consumers are done with them.  The stages this
+                // thread still owes an arrival are published first (the consumers finish the previous run only with them).
+                cp_async_wait<0>();
+                fence_proxy_async();
+                for (; arrived < it; ++arrived) mbar_arrive(full_a(arrived % p.stages));
+                ++wrun; cur_k = k; cur_pass = pass;
+                if (wrun >= 1) mbar_wait(w_empty, (wrun - 1) & 1);
+                const unsigned char* src = p.wpacked + PACK_HEADER + (size_t)k * w_bytes;
+                mbar_expect_tx(w_full, w_bytes);
+                for (int c = 0; c < p.nchunks; ++c) bulk_g2s(base + (uint32_t)c * 2u * b_tile, src + (size_t)c * 2u * b_tile, 2u * b_tile, w_full);
+            }
             const bool use_h = (p.in1_h[pass] != nullptr) && (p.c2 == 0 || p.in2_h[pass] != nullptr);
-            any_h |= use_h;
             int src[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) { const int r = rbase + 16 * j; src[j] = r < cnt ? __ldg(p.pair_in + pbase + r) : -1; }
-            for (int c = 0; c < p.nchunks; ++c, ++it) {
+            for (int c = 0; c < p.nchunks; ++c) {
                 const int s = it % p.stages;
                 mbar_wait(empty_a(s), ((it / p.stages) & 1) ^ 1);
                 unsigned char* a_hi = a_gen + (size_t)s * a_stage;
@@ -127,9 +127,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_scatter(const Params p) {
                     if (use_h) produce_a_split(reinterpret_cast<const __half*>(first ? p.in1_h[pass] : p.in2_h[pass]), cw, co, src, a_hi_u, a_hi_u + A_TILE, rbase, sub);
                     else produce_a_f32(first ? p.in1[pass] : p.in2[pass], cw, co, src, a_hi, a_hi + A_TILE, rbase, sub);
                 }
-                // one protocol for both paths: a cp.async group per stage (empty for the fp32 path), arrive D stages later
+                // one protocol for both paths: a cp.async group per stage (empty for the fp32 path), published D stages later
                 cp_async_commit();
-                if (it >= D) {
+                ++it;
+                if (it - arrived > D) {
                     cp_async_wait_dyn(D);
                     fence_proxy_async();
                     mbar_arrive(full_a(arrived % p.stages));
@@ -140,113 +141,58 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_scatter(const Params p) {
         cp_async_wait<0>();
         fence_proxy_async();
         for (; arrived < it; ++arrived) mbar_arrive(full_a(arrived % p.stages));
-        (void)any_h;
-    } else if (warp == 4) {
-        // =========================== MMA issuer ===========================
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc(p.cout);
-            int it = 0, j = 0, wrun = -1, cur_k = -1, cur_pass = -1;
-            for (int T = t_begin; T < t_end; ++T, ++j) {
-                int pass, k, pbase, cnt;
-                decode(T, pass, k, pbase, cnt);
-                if (k != cur_k || pass != cur_pass) {              // new run of equal k: its weights must have landed
-                    ++wrun; cur_k = k; cur_pass = pass;
-                    mbar_wait(w_full, wrun & 1);
-                    tc_fence_after();
-                }
-                const int buf = j & 1;
-                if (j >= 2) { mbar_wait(acc_empty(buf), ((j >> 1) - 1) & 1); tc_fence_after(); }
-                const uint32_t tmem_acc = tmem_d + (uint32_t)(buf * p.acc_stride);
-                for (int c = 0; c < p.nchunks; ++c, ++it) {
-                    const int s = it % p.stages;
-                    mbar_wait(full_a(s), (it / p.stages) & 1);
-                    tc_fence_after();
-                    const uint32_t a_hi = a_base + (uint32_t)s * a_stage, a_lo = a_hi + A_TILE;
-                    const uint32_t b_hi = base + (uint32_t)c * 2u * b_tile, b_lo = b_hi + b_tile;
-                    const int ksteps = min(KC, ctot - c * KC) >> 4;
-                    for (int ks = 0; ks < ksteps; ++ks) {
-                        const uint64_t dah = make_desc(a_hi + ks * 32), dal = make_desc(a_lo + ks * 32);
-                        const uint64_t dbh = make_desc(b_hi + ks * 32), dbl = make_desc(b_lo + ks * 32);
-                        umma(tmem_acc, dah, dbh, idesc, (c | ks) ? 1u : 0u);
-                        umma(tmem_acc, dal, dbh, idesc, 1);
-                        umma(tmem_acc, dah, dbl, idesc, 1);
-                    }
-                    umma_commit(empty_a(s));
-                }
-                umma_commit(acc_full(buf));
-                // last tile of this run of equal k?  then the weights may be replaced once these MMAs are done
-                bool run_ends = (T + 1 == t_end);
-                if (!run_ends) {
-                    int p2, k2, pb2, c2;
-                    decode(T + 1, p2, k2, pb2, c2);
-                    run_ends = (k2 != k) || (p2 != pass);
-                }
-                if (run_ends) umma_commit(w_empty);
-            }
-        }
-        __syncwarp();
-    } else if (warp == 5) {
-        // =========================== weight loader ===========================
-        if (lane == 0) {
-            int wrun = -1, cur_k = -1, cur_pass = -1;
-            for (int T = t_begin; T < t_end; ++T) {
-                int pass, k, pbase, cnt;
-                decode(T, pass, k, pbase, cnt);
-                if (k == cur_k && pass == cur_pass) continue;
-                ++wrun; cur_k = k; cur_pass = pass;
-                if (wrun >= 1) mbar_wait(w_empty, (wrun - 1) & 1);
-                const unsigned char* src = p.wpacked + PACK_HEADER + (size_t)k * w_bytes;
-                mbar_expect_tx(w_full, w_bytes);
-                for (int c = 0; c < p.nchunks; ++c) bulk_g2s(base + (uint32_t)c * 2u * b_tile, src + (size_t)c * 2u * b_tile, 2u * b_tile, w_full);
-            }
-        }
-        __syncwarp();
     } else {
-        // =========================== scatter epilogue ===========================
-        // per 32-column slab: TMEM -> registers -> the warp's smem slab (transpose) -> lanes along channels, so each
-        // red.global.add.v4.f32 instruction covers 4 rows x 128 contiguous bytes (full sectors) instead of 32 rows x 16 B
-        const int q4 = warp & 3;
+        // =========================== consumers: wgmma, then red.add into out[pair_out] ===========================
+        const int wg = (warp >> 2) - 1;
         const float out_scale = __ldg(reinterpret_cast<const float*>(p.wpacked) + 1);
-        const uint32_t lane_base = (uint32_t)(q4 * 32) << 16;
-        float* myslab = slab + (size_t)q4 * 32 * SLAB_PITCH;
-        int j = 0;
-        for (int T = t_begin; T < t_end; ++T, ++j) {
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread's tile rows: r0 and r0 + 8
+        float acc[N / 2];
+        int it = 0, wrun = -1, cur_k = -1, cur_pass = -1;
+        for (int T = t_begin; T < t_end; ++T) {
             int pass, k, pbase, cnt;
             decode(T, pass, k, pbase, cnt);
-            const int r = q4 * 32 + lane;
-            const int orow = r < cnt ? __ldg(p.pair_out + pbase + r) : -1;
-            const int buf = j & 1;
-            mbar_wait(acc_full(buf), (j >> 1) & 1);
-            tc_fence_after();
-            for (int c0 = 0; c0 < p.cout; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(tmem_d + lane_base + (uint32_t)(buf * p.acc_stride + c0), v);
-                tmem_ld_wait();
-                __syncwarp();
-                float* srow = myslab + lane * SLAB_PITCH;
-#pragma unroll
-                for (int q = 0; q < 8; ++q)
-                    *reinterpret_cast<float4*>(srow + q * 4) = make_float4(__uint_as_float(v[q * 4]) * out_scale, __uint_as_float(v[q * 4 + 1]) * out_scale,
-                                                                           __uint_as_float(v[q * 4 + 2]) * out_scale, __uint_as_float(v[q * 4 + 3]) * out_scale);
-                __syncwarp();
-#pragma unroll
-                for (int e = lane; e < 256; e += 32) {
-                    const int rr = e >> 3, c4 = (e & 7) * 4;
-                    const int dst_row = __shfl_sync(0xffffffffu, orow, rr);
-                    if (dst_row >= 0) {
-                        const float4 a4 = *reinterpret_cast<const float4*>(myslab + rr * SLAB_PITCH + c4);
-                        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p.out[pass] + (long long)dst_row * p.cout + c0 + c4),
-                                     "f"(a4.x), "f"(a4.y), "f"(a4.z), "f"(a4.w) : "memory");
-                    }
-                }
+            if (k != cur_k || pass != cur_pass) {              // new run of equal k: its weights must have landed
+                ++wrun; cur_k = k; cur_pass = pass;
+                mbar_wait(w_full, wrun & 1);
             }
-            tc_fence_before();
-            mbar_arrive(acc_empty(buf));
+            const int orow0 = r0 < cnt ? __ldg(p.pair_out + pbase + r0) : -1;
+            const int orow1 = r0 + 8 < cnt ? __ldg(p.pair_out + pbase + r0 + 8) : -1;
+            int prev_s = -1;
+            for (int c = 0; c < p.nchunks; ++c, ++it) {
+                const int s = it % p.stages;
+                mbar_wait(full_a(s), (it / p.stages) & 1);
+                const uint32_t a_hi = a_base + (uint32_t)s * a_stage + (uint32_t)wg * (A_TILE / 2), a_lo = a_hi + A_TILE;
+                const uint32_t b_hi = base + (uint32_t)c * 2u * b_tile, b_lo = b_hi + b_tile;
+                const int ksteps = min(KC, ctot - c * KC) >> 4;
+                reg_fence(acc);
+                wg_stage_mma<N>(acc, a_hi, a_lo, b_hi, b_lo, ksteps, c == 0);
+                reg_fence(acc);
+                wgmma_wait<1>();
+                if (prev_s >= 0 && lane == 0) mbar_arrive(empty_a(prev_s));
+                prev_s = s;
+            }
+            wgmma_wait<0>();
+            reg_fence(acc);
+            if (lane == 0) mbar_arrive(empty_a(prev_s));
+            // last tile of this run of equal k?  then the weights may be replaced
+            bool run_ends = (T + 1 == t_end);
+            if (!run_ends) {
+                int p2, k2, pb2, c2;
+                decode(T + 1, p2, k2, pb2, c2);
+                run_ends = (k2 != k) || (p2 != pass);
+            }
+            if (run_ends && lane == 0) mbar_arrive(w_empty);
+            float* out = p.out[pass];
+#pragma unroll
+            for (int i = 0; i < N / 2; i += 2) {
+                const int orow = ((i >> 1) & 1) ? orow1 : orow0;
+                if (orow < 0) continue;
+                const int col = 8 * (i >> 2) + 2 * (lane & 3);
+                asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(out + (long long)orow * p.cout + col),
+                             "f"(acc[i] * out_scale), "f"(acc[i + 1] * out_scale) : "memory");
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"((uint32_t)p.tmem_cols) : "memory");
 }
 
 // ---- pair lists of a kernel map, grouped by offset ------------------------------------------------------------------
@@ -297,7 +243,16 @@ __global__ void k_zero_rows(float* __restrict__ buf, const int* __restrict__ d_n
 
 static size_t smem_bytes(int cin, int cout, int stages) {
     const int nchunks = (cin + tc::KC - 1) / tc::KC;
-    return 1024 + (size_t)nchunks * 2 * cout * 128 + (size_t)stages * 2 * tc::A_TILE + SLAB_BYTES + (2 * MAX_STAGES + 6) * 8 + 64;
+    return 1024 + (size_t)nchunks * 2 * cout * 128 + (size_t)stages * 2 * tc::A_TILE;
+}
+
+template <int N>
+static int launch(Lb2Handle* h, cudaStream_t s, const Params& p, size_t smem) {
+    cudaError_t e = lb2_configure_smem(h, LB2_K_SCATTER + (N / 32 - 1), k_spconv_scatter<N>, (int)(227 * 1024 - 512));   // static smem: bars + offsets
+    if (e != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "k_spconv_scatter smem attribute: %s", cudaGetErrorString(e));
+    k_spconv_scatter<N><<<h->num_sms, THREADS, smem, s>>>(p);
+    LB2_POST_LAUNCH(h, "k_spconv_scatter");
+    return LB2_OK;
 }
 
 static bool shape_ok(int c1, int c2, int cout, int kvol) {
@@ -305,7 +260,7 @@ static bool shape_ok(int c1, int c2, int cout, int kvol) {
     if (kvol < 1 || kvol > MAX_KVOL || ctot % 16 || ctot < 16) return false;
     if (c2 > 0 && (c1 % 8 || c2 % 8)) return false;
     if (cout % 32 || cout < 32 || cout > 128) return false;
-    return smem_bytes(ctot, cout, 2) <= 227 * 1024 - 256;
+    return smem_bytes(ctot, cout, 2) <= 227 * 1024 - 512;
 }
 
 }  // namespace sc
@@ -351,21 +306,19 @@ extern "C" int lb2_spconv_scatter(void* handle, void* stream, const lb2_scatter_
         p.in1_h[i] = d->in1_h[j]; p.in2_h[i] = d->in2_h[j];
     }
     int stages = sc::MAX_STAGES;
-    while (stages > 2 && sc::smem_bytes(d->c1 + d->c2, d->cout, stages) > 227 * 1024 - 256) --stages;
+    while (stages > 2 && sc::smem_bytes(d->c1 + d->c2, d->cout, stages) > 227 * 1024 - 512) --stages;
     p.stages = stages;
-    const int half = d->cout <= 32 ? 32 : d->cout <= 64 ? 64 : 128;
-    p.acc_stride = half; p.tmem_cols = 2 * half;
     if (d->zero_rows_cap > 0) {        // clear the rows the scatter adds into
         for (int i = 0; i < d->npass; ++i) {
             sc::k_zero_rows<<<cdiv((long long)d->zero_rows_cap * d->cout / 4, 256), 256, 0, s>>>(d->out[i], d->d_zero_rows, d->zero_rows_cap, d->cout);
             LB2_POST_LAUNCH(h, "k_zero_rows");
         }
     }
-    {
-        cudaError_t e = lb2_configure_smem(h, LB2_K_SCATTER, sc::k_spconv_scatter, (int)(227 * 1024 - 256));   // 224 B of static smem
-        if (e != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "k_spconv_scatter smem attribute: %s", cudaGetErrorString(e));
+    const size_t smem = sc::smem_bytes(d->c1 + d->c2, d->cout, stages);
+    switch (d->cout) {
+        case 32: return sc::launch<32>(h, s, p, smem);
+        case 64: return sc::launch<64>(h, s, p, smem);
+        case 96: return sc::launch<96>(h, s, p, smem);
+        default: return sc::launch<128>(h, s, p, smem);
     }
-    sc::k_spconv_scatter<<<h->num_sms, sc::THREADS, sc::smem_bytes(d->c1 + d->c2, d->cout, stages), s>>>(p);
-    LB2_POST_LAUNCH(h, "k_spconv_scatter");
-    return LB2_OK;
 }

@@ -1,12 +1,12 @@
-// Device helpers shared by the tcgen05 kernels (spconv_tc.cu, spconv_scatter.cu): mbarrier / bulk-TMA / tcgen05
-// PTX wrappers, UMMA descriptors, the K-major SWIZZLE_128B addressing and the fp32 -> fp16 hi/lo split.
+// Device helpers shared by the wgmma kernels (spconv_tc.cu, spconv_scatter.cu): mbarrier / bulk-TMA / wgmma
+// PTX wrappers, GMMA shared-memory descriptors, the K-major SWIZZLE_128B addressing and the fp32 -> fp16 hi/lo split.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
 
 namespace tc {
 
-constexpr int BM = 128;              // rows per MMA tile (UMMA M)
+constexpr int BM = 128;              // rows per tile (two consumer warpgroups of wgmma M = 64)
 constexpr int KC = 64;               // channels per pipeline stage (one 128-byte swizzle atom of fp16)
 constexpr int A_TILE = BM * KC * 2;  // bytes of one fp16 A tile (hi or lo): 16 KB
 constexpr int PACK_HEADER = 256;     // packed weights: [0] max|W| bits, [1] 2^-k output scale
@@ -37,63 +37,77 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
+// K-major SWIZZLE_128B shared-memory matrix descriptor of wgmma (cute::GMMA::GmmaDescriptor):
 //   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (8 rows x 128 B = 1024 B)
-//   [46,48) version = 1 | [61,64) layout = 2 (SWIZZLE_128B)
+//   [49,52) base offset = 0 (tiles are 1024-byte aligned) | [62,64) layout = 1 (SWIZZLE_128B)
+// A step of 16 channels inside the 128-byte swizzle atom advances the start address by 32 bytes.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 (bits 4-5 = 1), A=B=f16 (formats 0),
-// both K-major, N>>3 at [17,23), M>>4 at [24,29)
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D(64 x n, fp32 registers) (+)= A(64 x 16, smem) . B(n x 16, smem)^T, both operands fp16 K-major.  accumulate = 0 overwrites D.
+// Register i of the calling thread (warp w, lane l of the warpgroup) holds row 16 w + l / 4 + 8 ((i / 2) & 1),
+// column 8 (i / 4) + 2 (l % 4) + (i & 1).
+__device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ void wgmma_m64n32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-// one lane of the (converged) calling warp
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
 
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
+// D(64 x N) for N a multiple of 16: n64 / n32 / n16 instructions side by side, B rows (= output channels) advance 128 bytes each
+template <int N, int OFF = 0>
+__device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint32_t b_addr, uint32_t accumulate) {
+    constexpr int REST = N - OFF;
+    if constexpr (REST >= 64) {
+        wgmma_m64n64(d + OFF / 2, da, make_desc(b_addr + OFF * 128), accumulate);
+        wgmma_n<N, OFF + 64>(d, da, b_addr, accumulate);
+    } else if constexpr (REST >= 32) {
+        wgmma_m64n32(d + OFF / 2, da, make_desc(b_addr + OFF * 128), accumulate);
+        wgmma_n<N, OFF + 32>(d, da, b_addr, accumulate);
+    } else if constexpr (REST >= 16) {
+        wgmma_m64n16(d + OFF / 2, da, make_desc(b_addr + OFF * 128), accumulate);
+    }
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
+// one pipeline stage of the FP16x3 product for the calling warpgroup: rows [64 wg, +64) of the A tiles (hi, lo) times the N rows of
+// the B tiles (hi, lo), ksteps 16-channel steps, 3 MMAs each (x_hi.w_hi + x_lo.w_hi + x_hi.w_lo); first = overwrite D
+template <int N>
+__device__ __forceinline__ void wg_stage_mma(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int ksteps, bool first) {
+    wgmma_fence();
+#pragma unroll 1
+    for (int ks = 0; ks < ksteps; ++ks) {
+        const uint64_t dah = make_desc(a_hi + ks * 32), dal = make_desc(a_lo + ks * 32);
+        wgmma_n<N>(d, dah, b_hi + ks * 32, (first && ks == 0) ? 0u : 1u);
+        wgmma_n<N>(d, dal, b_hi + ks * 32, 1u);
+        wgmma_n<N>(d, dah, b_lo + ks * 32, 1u);
+    }
+    wgmma_commit();
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-                 "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-                 "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-                 :: "r"(taddr),
-                    "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-                    "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-                    "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-                    "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-                 : "memory");
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {      // keeps the compiler from moving accumulator accesses across a wgmma wait
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // byte offset of (row, 16-byte chunk) inside a K-major SWIZZLE_128B tile (rows of 128 B, Swizzle<3,4,3>)
@@ -137,33 +151,6 @@ __device__ __forceinline__ void store_split4(void* base, long long row, int c, i
     *reinterpret_cast<uint2*>(rp + col) = uh;
     *reinterpret_cast<uint2*>(rp + c + col) = ul;
 }
-// write 4 consecutive channels of a split companion row: hi halfs at rp, lo halfs at rp + c (rp = row start + column, in halfs;
-// c = channels of the tensor).  Epilogue stores are evict-first (st.global.cs): an output streams through L2 instead of displacing
-// the feature rows the gathers re-read
-__device__ __forceinline__ void store_split4_at(__half* rp, int c, const float (&y)[4]) {
-    uint2 uh, ul;
-    split2(y[0], y[1], uh.x, ul.x);
-    split2(y[2], y[3], uh.y, ul.y);
-    __stcs(reinterpret_cast<uint2*>(rp), uh);
-    __stcs(reinterpret_cast<uint2*>(rp + c), ul);
-}
-__device__ __forceinline__ void store_f4(float* p, const float (&y)[4]) { __stcs(reinterpret_cast<float4*>(p), make_float4(y[0], y[1], y[2], y[3])); }
-
-// Ask L2 for the 128-byte lines of the epilogue operands of one output row (channels [c0, c0 + n) of a (rows, c) tensor): issued by
-// the drain warps when a tile's rows are known, long before the accumulator they belong to is complete, so the epilogue's loads hit L2
-// instead of paying the DRAM latency once per 16-channel slab.  `line` = which 128-byte line of the segment this lane asks for.
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-__device__ __forceinline__ void prefetch_row_f32(const float* base, long long row, int c, int c0, int n, int line) {
-    if (base && line * 32 < n) prefetch_l2(base + row * c + c0 + line * 32);
-}
-__device__ __forceinline__ void prefetch_row_split(const void* base_h, long long row, int c, int c0, int n, int line) {
-    if (base_h && line * 64 < n) {                       // hi and lo halves: n halfs each
-        const __half* rp = reinterpret_cast<const __half*>(base_h) + row * 2 * c + c0 + line * 64;
-        prefetch_l2(rp);
-        prefetch_l2(rp + c);
-    }
-}
-
 // 4 consecutive channels of a residual row: from the fp32 tensor, else from its split companion (hi + lo), else zero
 __device__ __forceinline__ float4 load_residual4(const float* res, const void* res_h, long long row, int c, int col) {
     if (res) return __ldg(reinterpret_cast<const float4*>(res + row * c + col));
@@ -175,201 +162,8 @@ __device__ __forceinline__ float4 load_residual4(const float* res, const void* r
     return make_float4(h0.x + l0.x, h0.y + l0.y, h1.x + l1.x, h1.y + l1.y);
 }
 
-// One 16-channel slab of a drain thread's register-resident totals -> its row of the warp's staging slab (raw accumulator units).  The slab index is a
-// template parameter (registers are addressed statically); the epilogue loops over the slabs at run time and dispatches through
-// slab_write_switch, so the global-memory part of the epilogue exists ONCE in the binary instead of once per slab (the fully unrolled
-// form made the kernels 85-185 KB of SASS and the drain warps stalled on instruction fetch, ncu: 'no_inst').
-template <int C, int TOT>
-__device__ __forceinline__ void slab_write(const float (&tot)[TOT], float* srow) {
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<float4*>(srow + q * 4) = make_float4(tot[C * 16 + q * 4], tot[C * 16 + q * 4 + 1], tot[C * 16 + q * 4 + 2], tot[C * 16 + q * 4 + 3]);
-}
-template <int TOT>
-__device__ __forceinline__ void slab_write_switch(int cs, const float (&tot)[TOT], float* srow) {
-    switch (cs) {
-        case 0: slab_write<0, TOT>(tot, srow); break;
-        case 1: if constexpr (TOT > 16) slab_write<1, TOT>(tot, srow); break;
-        case 2: if constexpr (TOT > 32) slab_write<2, TOT>(tot, srow); break;
-        case 3: if constexpr (TOT > 48) slab_write<3, TOT>(tot, srow); break;
-        case 4: if constexpr (TOT > 64) slab_write<4, TOT>(tot, srow); break;
-        case 5: if constexpr (TOT > 80) slab_write<5, TOT>(tot, srow); break;
-        case 6: if constexpr (TOT > 96) slab_write<6, TOT>(tot, srow); break;
-        default: if constexpr (TOT > 112) slab_write<7, TOT>(tot, srow); break;
-    }
-}
-
-// One finished accumulator (this lane's row, TOT columns from taddr) into the drain thread's running total.  First group of a tile:
-// all loads in flight, one wait, the registers simply become the total; later groups: chunk-wise round-to-nearest adds (the second level of
-// the two-level accumulation).
-template <int TOT>
-__device__ __forceinline__ void drain_acc(uint32_t taddr, float (&tot)[TOT], bool first) {
-    constexpr int W = (TOT % 32 == 0) ? 32 : 16;
-    if (first) {
-        uint32_t r[TOT / W][W];
-#pragma unroll
-        for (int cc = 0; cc < TOT / W; ++cc) {
-            if constexpr (W == 32) tmem_ld32(taddr + (uint32_t)(cc * W), r[cc]); else tmem_ld16(taddr + (uint32_t)(cc * W), r[cc]);
-        }
-        tmem_ld_wait();
-#pragma unroll
-        for (int cc = 0; cc < TOT / W; ++cc)
-#pragma unroll
-            for (int q = 0; q < W; ++q) tot[cc * W + q] = __uint_as_float(r[cc][q]);
-    } else {
-#pragma unroll
-        for (int cc = 0; cc < TOT / W; ++cc) {
-            uint32_t r[W];
-            if constexpr (W == 32) tmem_ld32(taddr + (uint32_t)(cc * W), r); else tmem_ld16(taddr + (uint32_t)(cc * W), r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int q = 0; q < W; ++q) tot[cc * W + q] = __fadd_rn(tot[cc * W + q], __uint_as_float(r[q]));
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// The epilogue of the register-total kernels (k_spconv_tc_small / _n256 / _pair), shared so every kernel rounds identically:
-//   y = ((acc * out_scale + pre_add) * bn_scale + bn_shift + residual), ReLU, then y and / or y * gate, each as fp32 and / or split
-//   (out_scale = 2^-k undoes the power-of-two scaling of the packed weights).
-// A drain warp holds TOT channels of its 32 rows (lane = row) and hands them to the memory system 16 channels at a time through its
-// staging slab, where lane l serves channels 4 (l & 3) .. +3 of rows (l >> 2) + 8 u, u = 0..3: 64 contiguous bytes per row and store.
-// What a pass reads and writes is folded into one flag word per tile; a slab iteration only executes the loads / adds / stores whose
-// flag is set (the common layer has none of the optional operands and one output form).  Offsets are 32-bit element indices: the
-// launchers refuse rows * 2 * Cout >= 2^32.
-// ---------------------------------------------------------------------------------------------------
-constexpr int EPI_PITCH = 20;                         // floats per slab row (16 + 4: conflict-free 16-byte accesses)
-enum : unsigned { EP_PRE = 1u, EP_RES32 = 2u, EP_RESH = 4u, EP_GATE = 8u, EP_OUT = 16u, EP_OUTH = 32u, EP_G = 64u, EP_GH = 128u,
-                  EP_RELU = 512u, EP_OPERANDS = EP_PRE | EP_RES32 | EP_RESH | EP_GATE };
-__device__ __forceinline__ unsigned epi_flags(const lb2_conv_io& io, int relu) {
-    unsigned f = 0;
-    if (io.pre_add) f |= EP_PRE;
-    if (io.residual) f |= EP_RES32; else if (io.residual_h) f |= EP_RESH;
-    if (io.out) f |= EP_OUT;
-    if (io.out_h) f |= EP_OUTH;
-    if (io.out_gated) f |= EP_G;
-    if (io.out_gated_h) f |= EP_GH;
-    if (io.gate_table && (f & (EP_G | EP_GH))) f |= EP_GATE;
-    if (relu) f |= EP_RELU;
-    return f;
-}
-__device__ __forceinline__ float4 load_split4_at(const __half* rp, int c) {     // hi + lo of 4 consecutive channels of a companion row
-    const uint2 uh = __ldg(reinterpret_cast<const uint2*>(rp)), ul = __ldg(reinterpret_cast<const uint2*>(rp + c));
-    const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&uh.x)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&uh.y));
-    const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&ul.x)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&ul.y));
-    return make_float4(h0.x + l0.x, h0.y + l0.y, h1.x + l1.x, h1.y + l1.y);
-}
-// the outputs of one row: y and / or y * gate, each as fp32 (element e of a (rows, C) tensor) and / or split (element eh of (rows, 2C))
-__device__ __forceinline__ void epi_store(float (&y)[4], const float4& gate, unsigned e, unsigned eh, int C, unsigned fl, const lb2_conv_io& io) {
-    if (fl & EP_OUT) store_f4(io.out + e, y);
-    if (fl & EP_OUTH) store_split4_at(reinterpret_cast<__half*>(io.out_h) + eh, C, y);
-    if (fl & (EP_G | EP_GH)) {
-        if (fl & EP_GATE) { y[0] *= gate.x; y[1] *= gate.y; y[2] *= gate.z; y[3] *= gate.w; }
-        if (fl & EP_G) store_f4(io.out_gated + e, y);
-        if (fl & EP_GH) store_split4_at(reinterpret_cast<__half*>(io.out_gated_h) + eh, C, y);
-    }
-}
-// The per-channel affine (eval-mode BN: scale, shift; identity when the caller passes none) staged once per CTA in shared memory as
-// aff_s[0..C) = scale, aff_s[C..2C) = shift: the epilogue reads it with LDS instead of a global load per 16-channel slab.
-__device__ __forceinline__ void stage_affine(float* aff_s, const float* __restrict__ scale, const float* __restrict__ shift, int C) {
-    for (int i = threadIdx.x; i < C; i += blockDim.x) {
-        aff_s[i] = scale ? __ldg(scale + i) : 1.f;
-        aff_s[C + i] = shift ? __ldg(shift + i) : 0.f;
-    }
-}
-// tot: this lane's row, channels [cb, cb + TOT) of C; orow / grow: output row and gate-table row of the 4 rows this lane serves
-// (orow < 0: no row).  RB = rows whose operand loads are in flight together (2 where the totals fill the registers).
-template <int TOT, int RB>
-__device__ __forceinline__ void epilogue_slabs(const float (&tot)[TOT], float* myslab, int lane, const int (&orow)[4], const int (&grow)[4],
-                                               int cb, int C, float out_scale, unsigned fl, const lb2_conv_io& io, const float* aff_s) {
-    constexpr unsigned NOROW = 0xffffffffu;
-    const float* srd = myslab + (lane >> 2) * EPI_PITCH + (lane & 3) * 4;
-    unsigned c0 = (unsigned)(cb + (lane & 3) * 4);                  // this lane's first channel of slab 0
-    unsigned e0[4];                                                 // element offset of (row u, c0) in a (rows, C) tensor
-#pragma unroll
-    for (int u = 0; u < 4; ++u) e0[u] = orow[u] >= 0 ? (unsigned)orow[u] * (unsigned)C + c0 : NOROW;
-    // opaque to the optimiser: under the drain warps' register pressure it otherwise re-derives these from the thread index and the
-    // row (6-10 instructions) in front of every load and store
-    asm volatile("" : "+r"(c0), "+r"(e0[0]), "+r"(e0[1]), "+r"(e0[2]), "+r"(e0[3]));
-#pragma unroll 1
-    for (int cs = 0; cs < TOT / 16; ++cs) {                    // run-time loop: one copy of the global-memory code (see slab_write_switch)
-        __syncwarp();
-        slab_write_switch<TOT>(cs, tot, myslab + lane * EPI_PITCH);
-        __syncwarp();
-        const unsigned col = c0 + 16u * (unsigned)cs;
-        float4 s4 = *reinterpret_cast<const float4*>(aff_s + col);                  // BN scale and shift of these 4 channels (stage_affine)
-        const float4 h4 = *reinterpret_cast<const float4*>(aff_s + C + col);
-        if (!(fl & EP_OPERANDS)) {
-            // ---- the common layer: no pre-add, residual or gate.  The weights' scale 2^-k (out_scale) goes into the BN scale: exact ----
-            s4.x *= out_scale; s4.y *= out_scale; s4.z *= out_scale; s4.w *= out_scale;
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                if (e0[u] == NOROW) continue;
-                const float4 a4 = *reinterpret_cast<const float4*>(srd + 8 * u * EPI_PITCH);
-                float y[4] = {fmaf(a4.x, s4.x, h4.x), fmaf(a4.y, s4.y, h4.y), fmaf(a4.z, s4.z, h4.z), fmaf(a4.w, s4.w, h4.w)};
-                if (fl & EP_RELU) {
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) y[q] = fmaxf(y[q], 0.f);
-                }
-                const unsigned e = e0[u] + 16u * (unsigned)cs;
-                epi_store(y, s4, e, 2u * e - col, C, fl, io);          // no gate on this path (EP_GATE clear): the argument is not read
-            }
-            continue;
-        }
-#pragma unroll
-        for (int u0 = 0; u0 < 4; u0 += RB) {                   // loads of RB rows first, then math + stores
-            float4 pre[RB], res[RB], gat[RB];
-            if (fl & EP_PRE) {
-#pragma unroll
-                for (int v = 0; v < RB; ++v)
-                    pre[v] = e0[u0 + v] != NOROW ? __ldg(reinterpret_cast<const float4*>(io.pre_add + (e0[u0 + v] + 16u * (unsigned)cs)))
-                                                 : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            if (fl & EP_RES32) {
-#pragma unroll
-                for (int v = 0; v < RB; ++v)
-                    res[v] = e0[u0 + v] != NOROW ? __ldg(reinterpret_cast<const float4*>(io.residual + (e0[u0 + v] + 16u * (unsigned)cs)))
-                                                 : make_float4(0.f, 0.f, 0.f, 0.f);
-            } else if (fl & EP_RESH) {
-#pragma unroll
-                for (int v = 0; v < RB; ++v)
-                    res[v] = e0[u0 + v] != NOROW ? load_split4_at(reinterpret_cast<const __half*>(io.residual_h) + (2u * (e0[u0 + v] + 16u * (unsigned)cs) - col), C)
-                                                 : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            if (fl & EP_GATE) {
-#pragma unroll
-                for (int v = 0; v < RB; ++v)
-                    gat[v] = e0[u0 + v] != NOROW ? __ldg(reinterpret_cast<const float4*>(io.gate_table + ((unsigned)grow[u0 + v] * (unsigned)C + col)))
-                                                 : make_float4(1.f, 1.f, 1.f, 1.f);
-            }
-#pragma unroll
-            for (int v = 0; v < RB; ++v) {
-                const int u = u0 + v;
-                if (e0[u] == NOROW) continue;
-                const float4 a4 = *reinterpret_cast<const float4*>(srd + 8 * u * EPI_PITCH);
-                float y[4] = {a4.x * out_scale, a4.y * out_scale, a4.z * out_scale, a4.w * out_scale};
-                if (fl & EP_PRE) { y[0] += pre[v].x; y[1] += pre[v].y; y[2] += pre[v].z; y[3] += pre[v].w; }
-                y[0] = fmaf(y[0], s4.x, h4.x); y[1] = fmaf(y[1], s4.y, h4.y); y[2] = fmaf(y[2], s4.z, h4.z); y[3] = fmaf(y[3], s4.w, h4.w);
-                if (fl & (EP_RES32 | EP_RESH)) { y[0] += res[v].x; y[1] += res[v].y; y[2] += res[v].z; y[3] += res[v].w; }
-                if (fl & EP_RELU) {
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) y[q] = fmaxf(y[q], 0.f);
-                }
-                const unsigned e = e0[u] + 16u * (unsigned)cs;
-                epi_store(y, gat[v], e, 2u * e - col, C, fl, io);
-            }
-        }
-    }
-}
-
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-// the calling thread's arrival on `bar` is triggered by the hardware once all its prior cp.async copies have landed (counts against the
-// barrier's expected arrivals): a stage is published the moment its last byte arrives, without the issuing thread waiting for it.
-// CUTLASS' own cp.async -> UMMA mainloop (sm100_mma_cpasync_warpspecialized.hpp) pairs exactly this with tcgen05.mma.
-__device__ __forceinline__ void cp_async_arrive_on(uint32_t bar) {
-    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>

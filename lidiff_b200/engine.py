@@ -1,5 +1,5 @@
 """Fused denoising engine: the sampling loop of
-/root/reference/lidiff/tools/diff_completion_pipeline.py:148-169 restructured for the B200
+/root/reference/lidiff/tools/diff_completion_pipeline.py:148-169 restructured for the H100
 (SURVEY.md App. D), every arithmetic step a call into the C-ABI CUDA library, no host
 synchronisation inside the loop (row counts stay in device scalars), buffers sized once.
 
@@ -124,7 +124,7 @@ class Geometry:
         self.nbr_dn = [None] + [torch.empty((8, n_cap), **i32) for _ in range(levels - 1)]
         self.nbr_up = [torch.empty((8, n_cap), **i32) for _ in range(levels - 1)] + [None] if with_up else None
         self.scratch = h.unique_scratch(n_cap)
-        self.counts = torch.empty(n_cap, **i32)
+        self.voxel_scratch = h.voxel_mean_scratch(n_cap, 3)             # level-0 features are the 3 point coordinates
         # (in,out) pair counters filled by lb2_kernel_map: [0:5] 3^3 per level, [5:9] stride-2 (out level 1..4),
         # [9:13] transposed (out level 0..3); [13:18] row counts per level (copied from d_n)
         self.pairs = torch.zeros(18, dtype=torch.int64, device=dev)
@@ -231,7 +231,8 @@ class Geometry:
                 map_up(l)
 
     def voxel_mean(self, feats, n_points, out):
-        self.h.voxel_mean(feats, self.inv[0], n_points, feats.shape[1], self.d_n[0], self.n_cap, out, self.counts)
+        assert feats.shape[1] == 3, "voxel_scratch is sized for 3-channel point features"
+        self.h.voxel_mean(feats, self.inv[0], n_points, 3, self.d_n[0], self.n_cap, out, self.voxel_scratch)
 
     def sizes(self):
         return [int(d.item()) for d in self.d_n]

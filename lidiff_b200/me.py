@@ -1,4 +1,4 @@
-"""MinkowskiEngine operator surface, B200-native underneath.
+"""MinkowskiEngine operator surface, H100-native underneath.
 
 Mirrors exactly the subset of `import MinkowskiEngine as ME` that the reference hot path uses
 (SURVEY.md 8b; call sites /root/reference/lidiff/models/minkunet.py:17-24,36-42,53-76,94-99,464,497
@@ -136,8 +136,7 @@ class TensorField:
         lvl = cm.levels[1]
         n, c = self._F.shape
         out = torch.empty((lvl.n, c), dtype=torch.float32, device=self.device)
-        counts = torch.empty(lvl.n, dtype=torch.int32, device=self.device)
-        cm.h.voxel_mean(self._F, cm.field_inverse, n, c, None, lvl.n, out, counts)
+        cm.h.voxel_mean(self._F, cm.field_inverse, n, c, None, lvl.n, out, cm.h.voxel_mean_scratch(lvl.n, c))
         return SparseTensor(out, coordinate_manager=cm, tensor_stride=1)
 
 
@@ -243,7 +242,7 @@ class _ConvBase(nn.Module):
             self.kernel.data.uniform_(-stdv, stdv)
 
     def _packed_weight(self, h):
-        """tensor-core image of the kernel (fp16 hi/lo, UMMA layout), cached until the parameter changes"""
+        """tensor-core image of the kernel (fp16 hi/lo, wgmma layout), cached until the parameter changes"""
         if getattr(self, "algo", _lib.ALGO_AUTO) == _lib.ALGO_FFMA:
             return None
         W = self.kernel

@@ -1,4 +1,4 @@
-"""`import MinkowskiEngine as ME` -> lidiff_b200.me (B200-native operator surface)."""
+"""`import MinkowskiEngine as ME` -> lidiff_b200.me (H100-native operator surface)."""
 from lidiff_b200.me import *  # noqa: F401,F403
 from lidiff_b200.me import (CoordinateManager, MinkowskiAlgorithm, MinkowskiBatchNorm, MinkowskiConvolution,  # noqa: F401
                             MinkowskiConvolutionTranspose, MinkowskiReLU, MinkowskiSyncBatchNorm, SparseTensor,

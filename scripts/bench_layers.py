@@ -1,4 +1,4 @@
-"""Per-layer timing of the sparse convolution variants (FFMA vs tcgen05) on the real 180k-point
+"""Per-layer timing of the sparse convolution variants (FFMA vs wgmma) on the real 180k-point
 geometry (development aid).  Usage: python scripts/bench_layers.py [sigma]"""
 import os
 import sys

@@ -1,6 +1,6 @@
 """CPU study (not collected by pytest; run `python scripts/numerics_split_study.py`) of how the operand split of the tensor-core
 convolution propagates through the 49-layer guided U-Net of the oracle.  Every scheme replaces the per-offset GEMM of
-oracle.me_cpu.conv by an emulation of the products the hardware would form (fp32 accumulation, RN — the TMEM truncation of the
+oracle.me_cpu.conv by an emulation of the products the hardware would form (fp32 accumulation, RN — the tensor-core truncation of the
 real kernels is a separate, measured effect, DESIGN.md §3), and reports the error of the guided eps against the fp64 network with
 the metric of tests/test_gpu_networks.py: max |a - b| / (|b| + rms(b)).
 Schemes:  fp32           plain fp32 GEMM (what the FFMA kernel and ME compute)

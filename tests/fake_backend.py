@@ -73,6 +73,9 @@ class FakeHandle:
     def unique_scratch(self, n_cap):
         return torch.empty(16, dtype=torch.uint8)
 
+    def voxel_mean_scratch(self, m_cap, c):
+        return torch.empty(16, dtype=torch.uint8)
+
     @staticmethod
     def _n(d_n, cap):
         return cap if d_n is None else min(int(d_n[0]), cap)
@@ -99,7 +102,7 @@ class FakeHandle:
         order = np.argsort(keys, kind="stable")
         self.grids[grid[0].data_ptr()] = (keys[order], order)
 
-    def voxel_mean(self, feats, inverse, n, c, d_m, m_cap, out, counts):
+    def voxel_mean(self, feats, inverse, n, c, d_m, m_cap, out, scratch):
         self.launches += 2
         M = self._n(d_m, m_cap)
         inv = inverse[:n].long()

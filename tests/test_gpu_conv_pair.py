@@ -1,8 +1,8 @@
-"""Direct parity of the engine-path tensor-core convolution kernels against the fp64 oracle: the kernels that need fp16 split
-companions (`in1_h` / `in2_h`: k_spconv_tc_n256, k_spconv_tc_small on the cp.async path, and the CTA-pair cta_group::2 kernel
-k_spconv_tc_pair) with the engine's row order, row masks, two guidance passes, concatenated inputs and the fused epilogue
-(BN affine + residual + ReLU + gate, fp32 and split outputs).  Every case runs once per kernel selection
-(lb2_set_option LB2_OPT_TC_PAIR = 0: single-CTA kernels, 2: pair kernel for Cout 128 and 256)."""
+"""Direct parity of the engine-path tensor-core convolution kernel against the fp64 oracle on its companion path (fp16 split
+inputs `in1_h` / `in2_h` gathered with cp.async), with the engine's row order, row masks, two guidance passes, concatenated inputs
+and the fused epilogue (BN affine + residual + ReLU + gate, fp32 and split outputs), for the Cout 128 and 256 layers of the
+coarse levels.  Every case runs through both ways a caller reaches the kernel: LB2_ALGO_AUTO (0, the library's dispatch picks the
+tensor-core variant for packed weights and a supported shape) and LB2_ALGO_TC (2, the tensor-core variant named directly)."""
 import numpy as np
 import pytest
 import torch
@@ -42,9 +42,9 @@ CASES = [  # c1, c2, cout, level of the output rows, map kind
 ]
 
 
-@pytest.mark.parametrize("pair", [0, 2])
+@pytest.mark.parametrize("algo", [0, 2])
 @pytest.mark.parametrize("c1,c2,cout,lvl,kind", CASES)
-def test_companion_path_kernels_match_fp64_oracle(geo, pair, c1, c2, cout, lvl, kind):
+def test_companion_path_kernels_match_fp64_oracle(geo, algo, c1, c2, cout, lvl, kind):
     from lidiff_b200 import _lib
     from lidiff_b200._lib import ConvDesc, ConvIO
     h, G, og, N = geo["h"], geo["G"], geo["og"], geo["n"]
@@ -92,13 +92,11 @@ def test_companion_path_kernels_match_fp64_oracle(geo, pair, c1, c2, cout, lvl, 
         d.io[p_] = ConvIO(dA[p_].data_ptr(), dB[p_].data_ptr() if dB is not None else None, dR[p_].data_ptr(), out[p_].data_ptr(),
                           dTab.data_ptr(), dGi.data_ptr() if p_ == 0 else None, outg[p_].data_ptr(), None,
                           A_h[p_].data_ptr(), B_h[p_].data_ptr() if B_h is not None else None, out_h[p_].data_ptr(), None)
-    old = h.get_option(_lib.OPT_TC_PAIR)
-    h.set_option(_lib.OPT_TC_PAIR, pair)
-    try:
-        h.spconv(d, _lib.ALGO_TC)
-        torch.cuda.synchronize()
-    finally:
-        h.set_option(_lib.OPT_TC_PAIR, old)
+    assert algo in (_lib.ALGO_AUTO, _lib.ALGO_TC)
+    l0 = h.launch_count()
+    h.spconv(d, algo)
+    torch.cuda.synchronize()
+    assert h.launch_count() - l0 == 1, "one conv launch (no split into a fallback path)"
     ts_in, ks, stride, tr = oconv
     for p_ in range(2):
         Fin = A[p_][:M_in] if B is None else torch.cat([A[p_][:M_in], B[p_][:M_in]], 1)
@@ -110,6 +108,6 @@ def test_companion_path_kernels_match_fp64_oracle(geo, pair, c1, c2, cout, lvl, 
         eg = rel_err(outg[p_][:M], y * gate.double())
         oh = out_h[p_][:M].float().cpu()
         es = rel_err(oh[:, :cout] + oh[:, cout:], y)
-        print(f"pair={pair} {c1}+{c2}->{cout} L{lvl} {kind} pass {p_}: rel err {e:.2e} gated {eg:.2e} split {es:.2e}")
+        print(f"algo={algo} {c1}+{c2}->{cout} L{lvl} {kind} pass {p_}: rel err {e:.2e} gated {eg:.2e} split {es:.2e}")
         assert e < 5e-5 and eg < 5e-5 and es < 5e-5, "tensor-core conv (companion path) vs fp64 oracle"
     assert out[:, M:].abs().sum() == 0, "rows beyond the live count must stay untouched"

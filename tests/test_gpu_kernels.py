@@ -577,8 +577,8 @@ def test_split_companion_inputs_give_identical_results(c1, c2, cout):
                                                     (256, 0, 256, 3, "up"), (128, 0, 128, 4, "dn"), (384, 0, 256, 3, "1"),
                                                     (64, 0, 64, 2, "3"), (128, 64, 128, 2, "3"), (64, 0, 128, 3, "3"), (32, 0, 64, 2, "1")])
 def test_persistent_kernel_equals_per_tile_kernel(c1, c2, cout, lvl, kind):
-    """LB2_ALGO_TC (persistent, cross-tile pipelined) and LB2_ALGO_TC_TILE (one CTA per tile) run the same math in the
-    same order: identical results, with row order, two passes, fused epilogue and split outputs"""
+    """LB2_ALGO_TC and LB2_ALGO_TC_TILE run the same math in the same order: identical results, with row order, two passes,
+    fused epilogue and split outputs"""
     from lidiff_b200 import _lib
     from lidiff_b200._lib import ConvDesc, ConvIO
     from lidiff_b200.engine import Geometry
@@ -611,9 +611,6 @@ def test_persistent_kernel_equals_per_tile_kernel(c1, c2, cout, lvl, kind):
         return xh
     A_h, B_h = split_of(A), split_of(B)                # with companions the 256-channel layers take the register-total kernel
     res = []
-    old_pair = h.get_option(_lib.OPT_TC_PAIR)
-    h.set_option(_lib.OPT_TC_PAIR, 0)          # the single-CTA persistent kernels; the CTA-pair kernel runs the union of two tiles' offsets
-                                               # (other accumulation grouping) and has its own oracle test (test_gpu_conv_pair.py)
     for algo in (_lib.ALGO_TC_TILE, _lib.ALGO_TC):
         out, outg = torch.zeros(2, N, cout, device=DEV), torch.zeros(2, N, cout, device=DEV)
         out_h = torch.zeros(2, N, 2 * cout, dtype=torch.float16, device=DEV)
@@ -631,7 +628,6 @@ def test_persistent_kernel_equals_per_tile_kernel(c1, c2, cout, lvl, kind):
                               A_h[p_].data_ptr(), B_h[p_].data_ptr() if B_h is not None else None, out_h[p_].data_ptr(), None)
         h.spconv(d, algo)
         res.append((out[:, :M].clone(), outg[:, :M].clone(), out_h[:, :M].clone()))
-    h.set_option(_lib.OPT_TC_PAIR, old_pair)
     for a, b in zip(res[0], res[1]):
         assert torch.equal(a, b)
     assert res[0][0].abs().sum() > 0

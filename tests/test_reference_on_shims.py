@@ -1,39 +1,28 @@
-"""The reference's OWN inference class executing on the import shims (SURVEY.md 8f-1, a16; VERDICT r1 item 8):
-`/root/reference/lidiff/tools/diff_completion_pipeline.py` is imported unchanged, `DiffCompletion(diff_path, refine_path, T, s)` is
-constructed from synthetic Lightning-format checkpoints (ctor :15-56: torch.load, save_hyperparameters, strict=False state-dict
-loads, scheduler construction, exp_config.yaml) and `complete_scan(points)` (:117-169) runs end to end — preprocess (open3d FPS),
-points_to_tensor, the guided sampling loop over the ME / diffusers shims, postprocess, refinement, 6x offsets — and equals this
-repo's mirror `lidiff_b200.pipeline.DiffCompletion` bit for bit under the same torch seed, for two consecutive scans (the reference
-never resets its scheduler between scans).
+"""The reference's OWN inference class on the import shims, against this repo's mirror `lidiff_b200.pipeline.DiffCompletion`:
+the reference's `lidiff/tools/diff_completion_pipeline.py`, imported unchanged, constructed `DiffCompletion(diff_path, refine_path, T, s)`
+from synthetic Lightning-format checkpoints (ctor: torch.load, save_hyperparameters, strict=False state-dict loads, scheduler
+construction, exp_config.yaml) and ran `complete_scan(points)` end to end — preprocess (open3d FPS), points_to_tensor, the guided
+sampling loop over the ME / diffusers shims, postprocess, refinement, 6x offsets — for two consecutive scans under torch seed 123
+(the reference never resets its scheduler between scans).  tests/golden/make_reference_goldens.py recorded that run in
+tests/golden/reference_on_shims.npz; the mirror must reproduce it bit for bit.
 
-The reference tree exists only in the build container (not on the GPU box) and this container has no GPU, so the CUDA library is
-replaced by tests/fake_backend.py (CPU stand-in under the same C-ABI-shaped handle) and `.cuda()` is a no-op: what runs is every
-line of the reference's host code and of the shims; the kernels themselves are covered by the -m gpu suites."""
-import importlib
+The CUDA library is replaced by tests/fake_backend.py (CPU stand-in under the same C-ABI-shaped handle) and `.cuda()` is a no-op:
+what runs is every line of the mirror's host code and of the shims; the kernels themselves are covered by the -m gpu suites."""
 import os
-import sys
 
 import numpy as np
-import pytest
 import torch
 
 import fake_backend
 from conftest import make_scan
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "lidiff/tools/diff_completion_pipeline.py")),
-                                reason="reference tree not mounted")
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_on_shims.npz")
 
 
-@pytest.fixture()
-def ref_module(monkeypatch, tmp_path):
-    import lidiff_b200.shims as sh
-    sh.install()
-    for m in ("open3d", "natsort", "pytorch_lightning", "MinkowskiEngine", "diffusers", "pykeops"):
-        for k in [k for k in sys.modules if k == m or k.startswith(m + ".")]:
-            sys.modules.pop(k)
-    fake_backend.install(monkeypatch)
-    monkeypatch.setattr(torch.Tensor, "cuda", lambda self, *a, **k: self)           # no GPU in this container
+def patch_for_cpu(monkeypatch, mod=None, cwd=None):
+    """CPU stand-ins for what the reference's host code expects of a CUDA machine; mod: the imported inference script (its open3d
+    farthest point sampling is a CUDA kernel in the shim, the oracle's CPU restatement stands in for it)"""
+    monkeypatch.setattr(torch.Tensor, "cuda", lambda self, *a, **k: self)
     monkeypatch.setattr(torch.nn.Module, "cuda", lambda self, *a, **k: self)
     orig_to = torch.Tensor.to
 
@@ -44,22 +33,15 @@ def ref_module(monkeypatch, tmp_path):
             k["device"] = torch.device("cpu")
         return orig_to(self, *a, **k)
     monkeypatch.setattr(torch.Tensor, "to", to_cpu_instead_of_cuda)
-    monkeypatch.chdir(tmp_path)                                                     # the ctor writes ./results/<exp>/exp_config.yaml
-    sys.path.insert(0, REF)
-    for k in [k for k in sys.modules if k == "lidiff" or k.startswith("lidiff.")]:
-        sys.modules.pop(k)
-    mod = importlib.import_module("lidiff.tools.diff_completion_pipeline")
-    # open3d's farthest point sampling is a CUDA kernel in the shim: here the oracle's CPU restatement stands in for it
-    from oracle.pipeline import farthest_point_sample as fps_cpu
+    if cwd is not None:
+        monkeypatch.chdir(cwd)                                                      # the ctor writes ./results/<exp>/exp_config.yaml
+    if mod is not None:
+        from oracle.pipeline import farthest_point_sample as fps_cpu
 
-    def fps(self, n):
-        pts = np.asarray(self.points)
-        return type(self)(pts[fps_cpu(pts, int(n))])
-    monkeypatch.setattr(mod.o3d.geometry.PointCloud, "farthest_point_down_sample", fps)
-    yield mod
-    sys.path.remove(REF)
-    for k in [k for k in sys.modules if k == "lidiff" or k.startswith("lidiff.")]:
-        sys.modules.pop(k)
+        def fps(self, n):
+            pts = np.asarray(self.points)
+            return type(self)(pts[fps_cpu(pts, int(n))])
+        monkeypatch.setattr(mod.o3d.geometry.PointCloud, "farthest_point_down_sample", fps)
 
 
 def lightning_checkpoints(tmp_path, n_points):
@@ -75,40 +57,33 @@ def lightning_checkpoints(tmp_path, n_points):
     sd_diff = {f"partial_enc.{k}": v for k, v in sds["enc"].items()}
     sd_diff.update({f"model.{k}": v for k, v in sds["diff"].items()})
     sd_ref = {f"model_refine.{k}": v for k, v in sds["refine"].items()}
-    d, r = str(tmp_path / "diff_net.ckpt"), str(tmp_path / "refine_net.ckpt")
+    d, r = os.path.join(str(tmp_path), "diff_net.ckpt"), os.path.join(str(tmp_path), "refine_net.ckpt")
     torch.save({"epoch": 19, "hyper_parameters": hp, "state_dict": sd_diff}, d)
     torch.save({"epoch": 5, "hyper_parameters": hp, "state_dict": sd_ref}, r)
     return d, r
 
 
-def test_reference_diffcompletion_runs_on_shims_and_equals_the_mirror(ref_module, tmp_path):
+def test_reference_diffcompletion_runs_on_shims_and_equals_the_mirror(monkeypatch, tmp_path):
     from lidiff_b200.pipeline import DiffCompletion as Mirror
     from lidiff_b200.synth import range_filter, synthetic_scan
+    fake_backend.install(monkeypatch)
+    patch_for_cpu(monkeypatch, cwd=tmp_path)
+    z = np.load(GOLD)
     n_points = 2000
     diff_path, refine_path = lightning_checkpoints(tmp_path, n_points)
     raw = synthetic_scan(9, beams=16, azimuths=256)                           # (4096, 3) incl. points the range filter drops
-    ref = ref_module.DiffCompletion(diff_path, refine_path, 2, 6.0)
-    assert os.path.exists(tmp_path / "results" / "diff_net_T2_s6.0" / "exp_config.yaml")
-    assert ref.hparams["diff"]["s_steps"] == 2 and ref.w_uncond == 6.0 and len(ref.dpm_scheduler.timesteps) == 2
-    assert type(ref.model).__module__ == "lidiff.models.minkunet"             # the reference's own network classes, on the ME shim
     mir = Mirror(diff_path, refine_path, 2, 6.0, device="cpu", engine=False)
     assert mir.hparams["data"]["num_points"] == n_points
-    pre = ref.preprocess_scan(raw)
+    pre = torch.from_numpy(z["pre"])                                          # the reference's preprocess_scan(raw)
     assert tuple(pre.shape) == (1, n_points, 3) and pre.dtype == torch.float64
     assert pre.shape[1] == range_filter(raw).shape[0] or pre.shape[1] == n_points
-    outs = []
-    for who in (ref, mir):
-        torch.manual_seed(123)
-        res = []
-        for scan_no in range(2):                                              # second scan: multistep state carried over (no reset)
-            if who is ref:
-                refined, post = who.complete_scan(raw)
-            else:
-                refined, post = who.complete_scan(pre, preprocessed=True)
-            assert refined.shape == (6 * post.shape[0], 3) and np.isfinite(refined).all() and post.shape[0] > 0
-            res.append((refined, post))
-        outs.append(res)
-    for (ra, pa), (rb, pb) in zip(*outs):
-        assert pa.shape == pb.shape and np.array_equal(pa, pb), "diffusion result: reference class on shims vs mirror"
-        assert np.array_equal(ra, rb), "refined result: reference class on shims vs mirror"
-    assert not np.array_equal(outs[0][0][1], outs[0][1][1])                   # the two scans drew different noise
+    torch.manual_seed(123)
+    res = []
+    for scan_no in range(2):                                                  # second scan: multistep state carried over (no reset)
+        refined, post = mir.complete_scan(pre, preprocessed=True)
+        assert refined.shape == (6 * post.shape[0], 3) and np.isfinite(refined).all() and post.shape[0] > 0
+        pa, ra = z[f"post{scan_no}"], z[f"refined{scan_no}"]
+        assert pa.shape == post.shape and np.array_equal(pa, post), "diffusion result: reference class on shims vs mirror"
+        assert np.array_equal(ra, refined), "refined result: reference class on shims vs mirror"
+        res.append(post)
+    assert not np.array_equal(res[0], res[1])                                 # the two scans drew different noise
