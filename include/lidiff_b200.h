@@ -297,6 +297,49 @@ int lb2_guidance_dpm_step(void* h, void* stream, const float* eps_c, const float
 int lb2_farthest_point_sample(void* h, void* stream, const double* pts, int32_t n, int32_t n_samples,
                               int32_t* out_idx, double* dist_scratch);
 
+/* ---- evaluation metrics — lidiff/utils/metrics.py:63-221, histogram_metrics.py:7-51, eval_path.py:65-170.
+ * Points are fp64 rows (n, 3).  Every result is deterministic: integer counts, fp64 sums in a fixed order. */
+
+/* Exact 1-NN point-to-cloud distance — replaces open3d PointCloud.compute_point_cloud_distance (KDTreeFlann 1-NN in fp64;
+ * metrics.py:70,131-132,153-156).  lb2_pc_tree_build sorts the reference cloud along a Morton curve and builds a box hierarchy
+ * over it (`tree`: lb2_pc_tree_bytes(n) bytes, n >= 1); lb2_pc_nn gives, for every query, dist[q] = sqrt(dx^2 + dy^2 + dz^2)
+ * (fp64, no FMA contraction) to its nearest reference point and, if idx != NULL, idx[q] = that point's index (lowest index on
+ * equal distances).  ~log(n) box tests per query, however far the query is from the cloud.
+ * scratch >= lb2_pc_nn_scratch_bytes(nq). */
+size_t lb2_pc_tree_bytes(int32_t n_cap);
+size_t lb2_pc_nn_scratch_bytes(int32_t nq_cap);
+int lb2_pc_tree_build(void* h, void* stream, const double* pts, int32_t n, void* tree);
+int lb2_pc_nn(void* h, void* stream, const double* q, int32_t nq, const void* tree, double* dist, int32_t* idx, void* scratch);
+
+/* np.histogramdd(pts, bins, range=[-50, 50]^3) binning (metrics.py:93-101, histogram_metrics.py:11): per axis
+ * bin = searchsorted(edges, x, 'right') - 1 with edges (bins + 1 fp64, np.linspace of the range) from the caller, a value equal
+ * to the last edge in the last bin, points outside the range on any axis dropped.  Outputs (each optional, cleared first):
+ * bits = occupancy bitset of bins^3 bits in C order (x slowest, z fastest; bit c at word c / 32, bit c % 32), counts = uint32
+ * per cell (bins^3), n_in = number of points inside the range.  bins <= 2048. */
+int lb2_voxel_occupancy(void* h, void* stream, const double* pts, int32_t n, const double* edges, int32_t bins,
+                        uint32_t* bits, uint32_t* counts, uint64_t* n_in);
+
+/* CompletionIoU confusion counts (metrics.py:103-105) of two occupancies of nbits cells:
+ * out[0] = tp = |gt & pred|, out[1] = fn = |gt & ~pred|, out[2] = fp = |~gt & pred|. */
+int lb2_occupancy_confusion(void* h, void* stream, const uint32_t* bits_gt, const uint32_t* bits_pred, int64_t nbits, uint64_t* out);
+
+/* BEV histogram of histogram_metrics.py:13,16 (counts clipped to 1, summed over z) from an occupancy of bins^3 cells:
+ * bev[x * bins + y] = number of occupied z cells of column (x, y). */
+int lb2_occupancy_bev(void* h, void* stream, const uint32_t* bits, int32_t bins, uint32_t* bev);
+
+/* Jensen-Shannon distance of two count histograms as histogram_metrics.py:15-44 computes it (normalise each by its sum, then
+ * scipy.spatial.distance.jensenshannon, natural log): *out = sqrt((sum rel_entr(p, m) + sum rel_entr(q, m)) / 2), m = (p + q) / 2;
+ * NaN if either histogram is empty.  scratch >= lb2_jsd_scratch_bytes(n). */
+size_t lb2_jsd_scratch_bytes(int64_t n);
+int lb2_jsd(void* h, void* stream, const uint32_t* hist_a, const uint32_t* hist_b, int64_t n, double* out, void* scratch);
+
+/* Per-direction distance statistics (RMSE / Chamfer means, metrics.py:72,134; precision / recall counts, metrics.py:158-165):
+ * *sum_out = fp64 sum of the n distances; counts_out[k] = number of distances < thresholds[k] (thresholds ascending, nt <= 4096).
+ * scratch >= lb2_dist_stats_scratch_bytes(nt). */
+size_t lb2_dist_stats_scratch_bytes(int32_t nt);
+int lb2_dist_stats(void* h, void* stream, const double* dist, int32_t n, const double* thresholds, int32_t nt,
+                   double* sum_out, uint64_t* counts_out, void* scratch);
+
 #ifdef __cplusplus
 }
 #endif

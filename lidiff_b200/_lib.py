@@ -65,6 +65,8 @@ EXPORTS = [
     "lb2_nn_table_bytes", "lb2_nn_table_build", "lb2_nn_match_table",
     "lb2_nn_tree_bytes", "lb2_nn_tree_build", "lb2_nn_match_tree",
     "lb2_pair_list", "lb2_pair_list_scratch_bytes", "lb2_spconv_scatter", "lb2_spconv_scatter_supported",
+    "lb2_pc_tree_bytes", "lb2_pc_nn_scratch_bytes", "lb2_pc_tree_build", "lb2_pc_nn", "lb2_voxel_occupancy", "lb2_occupancy_confusion",
+    "lb2_occupancy_bev", "lb2_jsd_scratch_bytes", "lb2_jsd", "lb2_dist_stats_scratch_bytes", "lb2_dist_stats",
 ]
 
 
@@ -132,6 +134,17 @@ class Lib:
         d.lb2_head_mlp.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, vp, i64, i64]
         d.lb2_guidance_dpm_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, DpmCoef, vp, vp, vp, vp]
         d.lb2_farthest_point_sample.argtypes = [vp, vp, vp, i32, i32, vp, vp]
+        for f, a in (("lb2_pc_tree_bytes", i32), ("lb2_pc_nn_scratch_bytes", i32), ("lb2_jsd_scratch_bytes", i64),
+                     ("lb2_dist_stats_scratch_bytes", i32)):
+            getattr(d, f).argtypes = [a]
+            getattr(d, f).restype = C.c_size_t
+        d.lb2_pc_tree_build.argtypes = [vp, vp, vp, i32, vp]
+        d.lb2_pc_nn.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp]
+        d.lb2_voxel_occupancy.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp, vp]
+        d.lb2_occupancy_confusion.argtypes = [vp, vp, vp, vp, i64, vp]
+        d.lb2_occupancy_bev.argtypes = [vp, vp, vp, i32, vp]
+        d.lb2_jsd.argtypes = [vp, vp, vp, vp, i64, vp, vp]
+        d.lb2_dist_stats.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -303,6 +316,47 @@ class Handle:
     def farthest_point_sample(self, pts, n, n_samples, out_idx, dist):
         self._check(self.dll.lb2_farthest_point_sample(self.hp, self._stream(), _ptr(pts), int(n), int(n_samples), _ptr(out_idx), _ptr(dist)),
                     "lb2_farthest_point_sample")
+
+    # -- evaluation metrics (fp64 (n, 3) contiguous point tensors) ---------------------------------------------------------------
+    def _bytes(self, nbytes):
+        return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=self.device)
+
+    def pc_tree(self, pts):
+        """Morton-sorted box hierarchy over the reference cloud `pts` for pc_nn"""
+        n = pts.shape[0]
+        tree = self._bytes(self.dll.lb2_pc_tree_bytes(n))
+        self._check(self.dll.lb2_pc_tree_build(self.hp, self._stream(), _ptr(pts), int(n), _ptr(tree)), "lb2_pc_tree_build")
+        return tree
+
+    def pc_nn(self, q, tree, dist, idx=None):
+        """dist[i] = distance of q[i] to its nearest point of the tree's cloud; idx[i] = that point (lowest index on ties)"""
+        nq = q.shape[0]
+        scratch = self._bytes(self.dll.lb2_pc_nn_scratch_bytes(nq))
+        self._check(self.dll.lb2_pc_nn(self.hp, self._stream(), _ptr(q), int(nq), _ptr(tree), _ptr(dist), _ptr(idx), _ptr(scratch)),
+                    "lb2_pc_nn")
+
+    def voxel_occupancy(self, pts, edges, bits=None, counts=None, n_in=None):
+        bins = edges.shape[0] - 1
+        self._check(self.dll.lb2_voxel_occupancy(self.hp, self._stream(), _ptr(pts), int(pts.shape[0]), _ptr(edges), int(bins), _ptr(bits),
+                                                 _ptr(counts), _ptr(n_in)), "lb2_voxel_occupancy")
+
+    def occupancy_confusion(self, bits_gt, bits_pred, nbits, out):
+        self._check(self.dll.lb2_occupancy_confusion(self.hp, self._stream(), _ptr(bits_gt), _ptr(bits_pred), int(nbits), _ptr(out)),
+                    "lb2_occupancy_confusion")
+
+    def occupancy_bev(self, bits, bins, bev):
+        self._check(self.dll.lb2_occupancy_bev(self.hp, self._stream(), _ptr(bits), int(bins), _ptr(bev)), "lb2_occupancy_bev")
+
+    def jsd(self, hist_a, hist_b, out):
+        n = hist_a.numel()
+        scratch = self._bytes(self.dll.lb2_jsd_scratch_bytes(n))
+        self._check(self.dll.lb2_jsd(self.hp, self._stream(), _ptr(hist_a), _ptr(hist_b), int(n), _ptr(out), _ptr(scratch)), "lb2_jsd")
+
+    def dist_stats(self, dist, thresholds, sum_out, counts_out):
+        nt = thresholds.shape[0]
+        scratch = self._bytes(self.dll.lb2_dist_stats_scratch_bytes(nt))
+        self._check(self.dll.lb2_dist_stats(self.hp, self._stream(), _ptr(dist), int(dist.shape[0]), _ptr(thresholds), int(nt), _ptr(sum_out),
+                                            _ptr(counts_out), _ptr(scratch)), "lb2_dist_stats")
 
 
 _LIB = None

@@ -44,6 +44,11 @@ static inline int lb2_fail(Lb2Handle* h, int code, const char* fmt, const char* 
 
 static inline unsigned cdiv(long long a, long long b) { return (unsigned)((a + b - 1) / b); }
 
+// stable radix sort of unsigned keys (coords.cu): order[i] = index of the i-th smallest of the first min(*d_n, n_cap) keys
+// (n_cap keys if d_n is NULL), ties in index order
+size_t rs_sort_scratch_bytes(int n_cap, int nbits);
+int rs_sort_keys(Lb2Handle* h, cudaStream_t s, const unsigned* keys, const int* d_n, int n_cap, int nbits, int* order, void* scratch);
+
 // ---------------------------------------------------------------------------------------------------
 // coordinate keys: 10 bit batch | 3 x 18 bit biased coordinate  (same packing as oracle/me_cpu.py)
 // ---------------------------------------------------------------------------------------------------

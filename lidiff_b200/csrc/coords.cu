@@ -692,6 +692,38 @@ extern "C" int lb2_row_order(void* handle, void* stream, const uint32_t* row_mas
     return LB2_OK;
 }
 
+// stable LSD sort of n unsigned keys of `nbits` significant bits (the point-cloud tree of metrics.cu sorts Morton codes with it):
+// order[i] = index of the i-th smallest key, equal keys in index order.  scratch >= rs_sort_scratch_bytes(n_cap, nbits).
+size_t rs_sort_scratch_bytes(int n_cap, int nbits) {
+    return ((size_t)RS_BINS * (rs_blocks(n_cap) + cdiv(nbits, RS_BITS)) + 4 * (size_t)n_cap) * sizeof(int);
+}
+
+int rs_sort_keys(Lb2Handle* h, cudaStream_t s, const unsigned* keys, const int* d_n, int n_cap, int nbits, int* order, void* scratch) {
+    const int nblk = rs_blocks(n_cap), npass = (int)cdiv(nbits, RS_BITS);
+    int* hist = (int*)scratch;
+    int* total = hist + (size_t)RS_BINS * nblk;
+    unsigned* keys_a = (unsigned*)(total + (size_t)npass * RS_BINS);
+    unsigned* keys_b = keys_a + n_cap;
+    int* vals_a = (int*)(keys_b + n_cap);
+    int* vals_b = vals_a + n_cap;
+    if (cudaMemsetAsync(total, 0, (size_t)npass * RS_BINS * sizeof(int), s) != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "rs_sort memset%s", "");
+    const unsigned* kin = keys;
+    const int* vin = nullptr;
+    for (int pass = 0; pass < npass; ++pass) {
+        const bool last = pass == npass - 1;
+        unsigned* kout = last ? nullptr : ((pass & 1) ? keys_b : keys_a);
+        int* vout = last ? order : ((pass & 1) ? vals_b : vals_a);
+        RsSrc src;
+        src.keys = kin; src.mask = nullptr; src.coords = nullptr; src.vals = vin; src.mode = 0; src.coord_shift = 0;
+        k_rs_hist<<<nblk, 256, 0, s>>>(src, d_n, n_cap, pass * RS_BITS, hist, total + pass * RS_BINS);
+        LB2_POST_LAUNCH(h, "k_rs_hist");
+        k_rs_scatter<<<nblk, 32 * RS_WARPS, 0, s>>>(src, d_n, n_cap, pass * RS_BITS, hist, total + pass * RS_BINS, kout, vout);
+        LB2_POST_LAUNCH(h, "k_rs_scatter");
+        kin = kout; vin = vout;
+    }
+    return LB2_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // nn tree: a bounding-volume hierarchy over the Morton-sorted keys of lb2_nn_match (built once per scan, the keys
 // are the conditioning scan's stride-16 voxels).  Complete binary tree in heap order over leaves of NT_LEAF

@@ -132,9 +132,15 @@ class PointCloud(Geometry):
 
     def compute_point_cloud_distance(self, target):
         """for every point of this cloud the Euclidean distance to its nearest point of `target` (open3d: KDTreeFlann 1-NN in
-        double precision) — what lidiff/utils/metrics.py builds RMSE / Chamfer distance / precision-recall on"""
+        double precision) — what lidiff/utils/metrics.py builds RMSE / Chamfer distance / precision-recall on.  On a GPU: the exact
+        fp64 tree search of the lidiff_b200 CUDA library (lidiff_b200.metrics.nn_distance)."""
         import torch
-        dev = "cuda" if torch.cuda.is_available() else "cpu"
+        if torch.cuda.is_available():
+            from lidiff_b200.metrics import nn_distance
+            if len(self._points) == 0 or len(target._points) == 0:
+                return np.zeros(len(self._points))
+            return nn_distance(np.asarray(self._points), np.asarray(target._points)).cpu().numpy()
+        dev = "cpu"
         q64 = torch.as_tensor(np.asarray(self._points), dtype=torch.float64, device=dev)
         r64 = torch.as_tensor(np.asarray(target._points), dtype=torch.float64, device=dev)
         if q64.shape[0] == 0 or r64.shape[0] == 0:

@@ -1,0 +1,199 @@
+"""Scores completed scans of a sequence — counterpart of the reference's
+`python lidiff/utils/eval_path.py -p PATH [-d diff.ckpt -r refine.ckpt -t 50 -s 6.0]` (lidiff/utils/eval_path.py:65-170): same
+options, the same per-scan lines and the same `res_log.yaml` (a JSON dict with jsd, jsd_noclip_3d, rmse_mean, rmse_std, ious,
+cd_mean, cd_std, pr, re, f1) next to --path, with every metric computed on the GPU (lidiff_b200.metrics).
+
+    python -m lidiff_b200.tools.eval_path -p results/exp/refine/ --data ./Datasets/SemanticKITTI/dataset/sequences/08
+    torchrun --nproc-per-node 8 -m lidiff_b200.tools.eval_path -p results/exp/ -d diff.ckpt -r refine.ckpt
+
+Two modes: with -d / -r (or --random-weights) every scan is completed with lidiff_b200.pipeline.DiffCompletion and the refined
+cloud is scored (--cloud diff scores the diffusion-only cloud); without them the `<stem>.ply` files in --path are scored, as
+lidiff_b200.tools.diff_completion_pipeline writes them.  Under torchrun scan b runs on rank b mod R; rank 0 folds the per-scan
+records in scan order, so the results do not depend on the number of ranks.
+"""
+from __future__ import annotations
+
+import json
+import os
+import re
+
+import click
+import numpy as np
+import torch
+
+from .. import metrics as M
+from ..sharding import gather_scans, scans_of_rank
+from ..shims.open3d.geometry import PointCloud, VoxelGrid
+from ..synth import read_ply_xyz
+
+PATH_DATA = "./Datasets/SemanticKITTI/dataset/sequences/08"
+
+
+def _rows_4x4(values):
+    pose = np.zeros((4, 4))
+    pose[0, :4], pose[1, :4], pose[2, :4] = values[0:4], values[4:8], values[8:12]
+    pose[3, 3] = 1.0
+    return pose
+
+
+def parse_calibration(filename: str) -> dict:
+    """KITTI calib.txt: `KEY: 12 numbers` per line -> {KEY: 4x4}"""
+    calib = {}
+    with open(filename) as f:
+        for line in f:
+            if not line.strip():
+                continue
+            key, content = line.strip().split(":")
+            calib[key] = _rows_4x4([float(v) for v in content.split()])
+    return calib
+
+
+def load_poses(calib_fname: str, poses_fname: str) -> list:
+    """poses.txt (12 numbers per line) in the LiDAR frame: Tr^-1 . pose . Tr when calib.txt exists"""
+    tr = parse_calibration(calib_fname)["Tr"] if os.path.exists(calib_fname) else None
+    poses = []
+    with open(poses_fname) as f:
+        for line in f:
+            if not line.strip():
+                continue
+            pose = _rows_4x4([float(v) for v in line.split()])
+            poses.append(np.linalg.inv(tr) @ (pose @ tr) if tr is not None else pose)
+    return poses
+
+
+def natural_sorted(names):
+    return sorted(names, key=lambda s: [int(t) if t.isdigit() else t for t in re.split(r"(\d+)", s)])
+
+
+def ground_truth(pose: np.ndarray, cur_scan: np.ndarray, seq_map: np.ndarray, max_range: float) -> np.ndarray:
+    """the map points within max_range of the pose, in the scan's frame, z in (-4, 4.4), inside the 10 m voxels the scan occupies"""
+    d = np.sum((seq_map - pose[:-1, -1]) ** 2, axis=-1) ** 0.5
+    gt = seq_map[d < max_range]
+    gt = (np.concatenate([gt, np.ones((gt.shape[0], 1))], -1) @ np.linalg.inv(pose).T)[:, :3]
+    gt = gt[(gt[:, 2] > -4.0) & (gt[:, 2] < 4.4)]
+    view = VoxelGrid.create_from_point_cloud(PointCloud(cur_scan), voxel_size=10.0)
+    return gt[np.asarray(view.check_if_included(gt), dtype=bool)]
+
+
+def scan_completion(data: str, scan_name: str, path: str, pipe, max_range: float, cloud: str):
+    """(prediction, the scan's points within max_range)"""
+    points = np.fromfile(os.path.join(data, "velodyne", scan_name), dtype=np.float32).reshape(-1, 4)
+    dist = np.sqrt(np.sum(points[:, :3] ** 2, axis=-1))
+    cur = points[dist < max_range, :3]
+    if pipe is None:
+        pred = read_ply_xyz(os.path.join(path, f"{scan_name.split('.')[0]}.ply"))
+        pred = pred[np.sqrt(np.sum(pred ** 2, axis=-1)) < max_range]
+    else:
+        refined, diff = pipe.complete_scan(points)
+        pred = refined if cloud == "refine" else diff
+    return pred, cur
+
+
+def score_scans(data: str, path: str, pipe, max_range: float, cloud: str, device, rank: int = 0, world: int = 1):
+    """(number of scans, {scan index: record as rows}) for the scans of this rank"""
+    poses = load_poses(os.path.join(data, "calib.txt"), os.path.join(data, "poses.txt"))
+    seq_map = np.load(os.path.join(data, "map_clean.npy"))
+    scans = natural_sorted(os.listdir(os.path.join(data, "velodyne")))
+    n = min(len(poses), len(scans))
+    local = {}
+    for b in scans_of_rank(n, world, rank):
+        pred, cur = scan_completion(data, scans[b], path, pipe, max_range, cloud)
+        gt = ground_truth(poses[b], cur, seq_map, max_range)
+        local[b] = M.record_to_rows(M.evaluate_scan(gt, pred, device=device))
+    return n, local
+
+
+def fold(records: dict, verbose: bool = True) -> dict:
+    """the metrics over the scans' records in scan order -> the res_log dict (prints the per-scan lines when verbose)"""
+    rmse, cd = M.RMSE(), M.ChamferDistance()
+    pr = M.PrecisionRecall(*M.PR_ARGS)
+    iou = M.CompletionIoU()
+    jsd_3d, jsd_bev = [], []
+    for b in sorted(records):
+        rec = records[b]
+        jsd_3d.append(rec.jsd_3d)
+        jsd_bev.append(rec.jsd_bev)
+        for acc in (rmse, iou, cd, pr):
+            acc.add(rec)
+        if verbose:
+            print(f"JSD 3D: {jsd_3d[-1]}")
+            print(f"JSD BEV: {jsd_bev[-1]}")
+            _print_totals(rmse, iou, cd, pr)
+    res = _totals(rmse, iou, cd, pr)
+    return {"jsd": np.array(jsd_bev).mean(), "jsd_noclip_3d": np.array(jsd_3d).mean(), "rmse_mean": res["rmse"][0], "rmse_std": res["rmse"][1],
+            "ious": res["ious"], "cd_mean": res["cd"][0], "cd_std": res["cd"][1], "pr": res["auc"][0], "re": res["auc"][1], "f1": res["auc"][2]}
+
+
+def _totals(rmse, iou, cd, pr):
+    return {"rmse": rmse.compute(), "ious": iou.compute(), "cd": cd.compute(), "auc": pr.compute_auc()}
+
+
+def _print_totals(rmse, iou, cd, pr):
+    t = _totals(rmse, iou, cd, pr)
+    print(f"RMSE Mean: {t['rmse'][0]}\tRMSE Std: {t['rmse'][1]}")
+    for v_size, v in t["ious"].items():
+        print(f"Voxel {v_size}cm IOU: {v}")
+    print(f"CD Mean: {t['cd'][0]}\tCD Std: {t['cd'][1]}")
+    print(f"Precision: {t['auc'][0]}\tRecall: {t['auc'][1]}\tF-Score: {t['auc'][2]}")
+
+
+def to_json(obj):
+    if isinstance(obj, dict):
+        return {str(k): to_json(v) for k, v in obj.items()}
+    return float(obj)
+
+
+def log_path(path: str) -> str:
+    """res_log.yaml in the directory of --path (its last component dropped, as the reference does)"""
+    return os.path.join(os.path.dirname(path) or ".", "res_log.yaml")
+
+
+@click.command()
+@click.option("--path", "-p", type=str, default="", help="path to the scan sequence (the .ply predictions when scoring files)")
+@click.option("--voxel_size", "-v", type=float, default=0.05, help="voxel size")
+@click.option("--max_range", "-m", type=float, default=50, help="max range")
+@click.option("--denoising_steps", "-t", type=int, default=50, help="number of denoising steps")
+@click.option("--cond_weight", "-s", type=float, default=6.0, help="conditioning weights")
+@click.option("--diff", "-d", type=str, default=None, help="run diffusion pipeline")
+@click.option("--refine", "-r", type=str, default=None, help="path to the checkpoint for refinement net")
+@click.option("--random-weights", is_flag=True, help="complete with seeded random parameters instead of checkpoints (plumbing)")
+@click.option("--data", type=str, default=PATH_DATA, help="sequence directory: velodyne/*.bin, calib.txt, poses.txt, map_clean.npy")
+@click.option("--cloud", type=click.Choice(["refine", "diff"]), default="refine", help="which completed cloud to score")
+def main(path, voxel_size, max_range, denoising_steps, cond_weight, diff, refine, random_weights, data, cloud):
+    rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
+    device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
+    torch.cuda.set_device(device)
+    if world > 1:
+        import torch.distributed as dist
+        dist.init_process_group("nccl", device_id=device)
+    pipe = None
+    if random_weights:
+        from ..pipeline import DiffCompletion
+        from ..weights import random_state_dict
+        sds = {k: random_state_dict(k, i) for i, k in enumerate(("enc", "diff", "refine"))}
+        pipe = DiffCompletion(state_dicts=sds, denoising_steps=denoising_steps, cond_weight=cond_weight, device=device)
+    elif diff is not None or refine is not None:
+        from ..pipeline import DiffCompletion
+        pipe = DiffCompletion(diff, refine, denoising_steps, cond_weight, device=device)
+    n, local = score_scans(data, path, pipe, max_range, cloud, device, rank, world)
+    gathered = gather_scans(local, n, device)
+    if rank == 0:
+        res = fold({b: M.record_from_rows(rows) for b, rows in gathered.items()})
+        print("\n\n=================== FINAL RESULTS ===================\n\n")
+        print(f"JSD 3D: {res['jsd_noclip_3d']}")
+        print(f"JSD BEV: {res['jsd']}")
+        print(f"RMSE Mean: {res['rmse_mean']}\tRMSE Std: {res['rmse_std']}")
+        for v_size, v in res["ious"].items():
+            print(f"Voxel {v_size}cm IOU: {v}")
+        print(f"CD Mean: {res['cd_mean']}\tCD Std: {res['cd_std']}")
+        print(f"Precision: {res['pr']}\tRecall: {res['re']}\tF-Score: {res['f1']}")
+        with open(log_path(path), "w") as f:
+            json.dump(to_json(res), f)
+    if world > 1:
+        import torch.distributed as dist
+        dist.barrier()
+        dist.destroy_process_group()
+
+
+if __name__ == "__main__":
+    main()
