@@ -340,6 +340,35 @@ size_t lb2_dist_stats_scratch_bytes(int32_t nt);
 int lb2_dist_stats(void* h, void* stream, const double* dist, int32_t n, const double* thresholds, int32_t nt,
                    double* sum_out, uint64_t* counts_out, void* scratch);
 
+/* ---- ground-truth maps — lidiff/map_from_scans.py:63-96 (the static map `<seq>/map_clean.npy` that the evaluation and the
+ * reference's dataloader read).  The reference appends every filtered, transformed scan to the map and de-duplicates the whole map
+ * again; since an existing map point always precedes a new scan in that concatenation, the result equals one global
+ * first-occurrence de-duplication over all scans, which these calls build scan by scan with a persistent table.
+ *
+ * The table is an lb2_grid used as a set of voxel keys: keys uint64[cap], vals int32[2 * cap] = [0, cap) claim (lowest point index
+ * of the call that created the slot), [cap, 2 cap) map row (-1 until the creating call has finished).  Key packing: 3 x 21 bit
+ * biased signed voxel indices (no batch field), i.e. +-2^20 voxels per axis (+-104 km at 0.1 m). */
+#define LB2_MAP_AXIS_BITS 21
+typedef struct { float m[12]; } lb2_pose;   /* rows 0..2 of the 4x4 scan-to-map pose, row-major, fp32 */
+
+/* lb2_map_rehash clears `table` (cap a power of two) and inserts the (key, row) pairs of old_table (keys NULL / cap 0: none), so a
+ * new table is made with old_table empty and a full one is grown into a larger one.  old_table.cap_table <= table.cap_table. */
+int lb2_map_rehash(void* h, void* stream, lb2_grid old_table, lb2_grid table);
+
+/* One scan: `points` (n, 4) fp32 rows x, y, z, remission; `labels` uint32[n] or NULL (no label filter).
+ *   keep     (l & 0xFFFF) in (1, 252)  and  sqrt_rn(((x^2 + y^2) + z^2) + r^2) > 3.5      (map_from_scans.py:74-85)
+ *   p'_k     ((m[4k] x + m[4k+1] y) + m[4k+2] z) + m[4k+3]  in fp32, every operation rounded (no FMA)   (:87-88, w = 1)
+ *   voxel    floor(p' / voxel_size): div_mode 0 true fp32 division (the reference's --cpu run), 1 multiply by fp32(1 / voxel_size)
+ *            (PyTorch's CUDA scalar division, its default device)
+ * A kept point whose voxel already has a map row is dropped; among the points of this call that share a new voxel the lowest index
+ * wins, and the winners are appended in point order as fp32 p' rows map[map_n ...].  d_out (device int32[2]): [0] = number of new
+ * rows, [1] = status, bit0 = a kept point's voxel index is outside the key range (that point is not inserted; the map is then
+ * incomplete and the caller should treat the build as failed).  n <= 4M; cap_table >= 2 * (map_n + n); map_cap >= map_n + n.
+ * Per-call work is O(n): nothing is cleared per call.  scratch >= lb2_map_scan_scratch_bytes(n). */
+size_t lb2_map_scan_scratch_bytes(int32_t n_cap);
+int lb2_map_scan(void* h, void* stream, const float* points, const uint32_t* labels, int32_t n, lb2_pose pose, float voxel_size,
+                 int32_t div_mode, lb2_grid table, float* map, int32_t map_n, int32_t map_cap, int32_t* d_out, void* scratch);
+
 #ifdef __cplusplus
 }
 #endif

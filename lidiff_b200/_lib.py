@@ -67,7 +67,12 @@ EXPORTS = [
     "lb2_pair_list", "lb2_pair_list_scratch_bytes", "lb2_spconv_scatter", "lb2_spconv_scatter_supported",
     "lb2_pc_tree_bytes", "lb2_pc_nn_scratch_bytes", "lb2_pc_tree_build", "lb2_pc_nn", "lb2_voxel_occupancy", "lb2_occupancy_confusion",
     "lb2_occupancy_bev", "lb2_jsd_scratch_bytes", "lb2_jsd", "lb2_dist_stats_scratch_bytes", "lb2_dist_stats",
+    "lb2_map_rehash", "lb2_map_scan_scratch_bytes", "lb2_map_scan",
 ]
+
+
+class Pose(C.Structure):
+    _fields_ = [("m", C.c_float * 12)]
 
 
 def _ptr(t):
@@ -145,6 +150,10 @@ class Lib:
         d.lb2_occupancy_bev.argtypes = [vp, vp, vp, i32, vp]
         d.lb2_jsd.argtypes = [vp, vp, vp, vp, i64, vp, vp]
         d.lb2_dist_stats.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp, vp]
+        d.lb2_map_rehash.argtypes = [vp, vp, Grid, Grid]
+        d.lb2_map_scan_scratch_bytes.argtypes = [i32]
+        d.lb2_map_scan_scratch_bytes.restype = C.c_size_t
+        d.lb2_map_scan.argtypes = [vp, vp, vp, vp, i32, Pose, f32, i32, Grid, vp, i32, i32, vp, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -357,6 +366,27 @@ class Handle:
         scratch = self._bytes(self.dll.lb2_dist_stats_scratch_bytes(nt))
         self._check(self.dll.lb2_dist_stats(self.hp, self._stream(), _ptr(dist), int(dist.shape[0]), _ptr(thresholds), int(nt), _ptr(sum_out),
                                             _ptr(counts_out), _ptr(scratch)), "lb2_dist_stats")
+
+    # -- ground-truth maps (lidiff_b200.maps) -------------------------------------------------------------------------------------
+    def new_map_table(self, cap: int):
+        """an empty voxel-key table of `cap` (a power of two) slots, in new_grid's (keys, vals, cap) form"""
+        return (torch.empty(cap, dtype=torch.int64, device=self.device), torch.empty(2 * cap, dtype=torch.int32, device=self.device), cap)
+
+    def map_rehash(self, old, table):
+        """clear `table` and insert the (key, row) pairs of `old` (None: none)"""
+        self._check(self.dll.lb2_map_rehash(self.hp, self._stream(), self._grid(old) if old is not None else Grid(None, None, 0),
+                                            self._grid(table)), "lb2_map_rehash")
+
+    def map_scan_scratch(self, n_cap: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_map_scan_scratch_bytes(int(n_cap)))
+
+    def map_scan(self, points, labels, pose12, voxel_size, div_mode, table, map_buf, map_n, out, scratch):
+        """filter, transform and insert the (n, 4) `points` (int32 / uint32 `labels` or None); out[0] = new rows appended to
+        map_buf[map_n:], out[1] = status (bit0: voxel index outside the key range)"""
+        pose = Pose((C.c_float * 12)(*[float(v) for v in pose12]))
+        self._check(self.dll.lb2_map_scan(self.hp, self._stream(), _ptr(points), _ptr(labels), int(points.shape[0]), pose, float(voxel_size),
+                                          int(div_mode), self._grid(table), _ptr(map_buf), int(map_n), int(map_buf.shape[0]), _ptr(out),
+                                          _ptr(scratch)), "lb2_map_scan")
 
 
 _LIB = None

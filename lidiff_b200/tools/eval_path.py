@@ -15,54 +15,18 @@ from __future__ import annotations
 
 import json
 import os
-import re
 
 import click
 import numpy as np
 import torch
 
 from .. import metrics as M
+from ..kitti import load_poses, natural_sorted, parse_calibration  # noqa: F401  (part of this module's interface)
 from ..sharding import gather_scans, scans_of_rank
 from ..shims.open3d.geometry import PointCloud, VoxelGrid
 from ..synth import read_ply_xyz
 
 PATH_DATA = "./Datasets/SemanticKITTI/dataset/sequences/08"
-
-
-def _rows_4x4(values):
-    pose = np.zeros((4, 4))
-    pose[0, :4], pose[1, :4], pose[2, :4] = values[0:4], values[4:8], values[8:12]
-    pose[3, 3] = 1.0
-    return pose
-
-
-def parse_calibration(filename: str) -> dict:
-    """KITTI calib.txt: `KEY: 12 numbers` per line -> {KEY: 4x4}"""
-    calib = {}
-    with open(filename) as f:
-        for line in f:
-            if not line.strip():
-                continue
-            key, content = line.strip().split(":")
-            calib[key] = _rows_4x4([float(v) for v in content.split()])
-    return calib
-
-
-def load_poses(calib_fname: str, poses_fname: str) -> list:
-    """poses.txt (12 numbers per line) in the LiDAR frame: Tr^-1 . pose . Tr when calib.txt exists"""
-    tr = parse_calibration(calib_fname)["Tr"] if os.path.exists(calib_fname) else None
-    poses = []
-    with open(poses_fname) as f:
-        for line in f:
-            if not line.strip():
-                continue
-            pose = _rows_4x4([float(v) for v in line.split()])
-            poses.append(np.linalg.inv(tr) @ (pose @ tr) if tr is not None else pose)
-    return poses
-
-
-def natural_sorted(names):
-    return sorted(names, key=lambda s: [int(t) if t.isdigit() else t for t in re.split(r"(\d+)", s)])
 
 
 def ground_truth(pose: np.ndarray, cur_scan: np.ndarray, seq_map: np.ndarray, max_range: float) -> np.ndarray:
