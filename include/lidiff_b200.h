@@ -114,8 +114,9 @@ int lb2_row_order(void* h, void* stream, const uint32_t* row_mask, const int32_t
 
 /* Cost order of the tiles of a map (scheduling only; results do not depend on it): order128[i] / order256[i] = index of the i-th most
  * expensive 128-row tile / 256-row super-tile of the row order `row_perm`, cost = number of kernel offsets the tile has to run (popcount of
- * the OR of its rows' masks); entries beyond the live tile count are -1.  A persistent convolution kernel can deal tiles to its CTAs in
- * snake order over this sequence (lb2_conv_desc.tile_order128 / tile_order256); the one-CTA-per-tile kernel of this build ignores it.
+ * the OR of its rows' masks); entries beyond the live tile count are -1.  The tensor-core convolution (lb2_conv_desc.tile_order128)
+ * launches its tiles in this order, most expensive first, so that the cheap tiles fill the tail of the launch; order256 is for a
+ * kernel that deals 256-row super-tiles to persistent CTAs and is not read by this build.
  * order128: cdiv(n_cap,128) ints, order256: cdiv(n_cap,256) ints, scratch: cdiv(n_cap,128) * 4 bytes. */
 int lb2_tile_order(void* h, void* stream, const uint32_t* row_mask, const int32_t* row_perm, const int32_t* d_n, int32_t n_cap,
                    int32_t* order128, int32_t* order256, void* scratch);
@@ -165,8 +166,10 @@ typedef struct {
                                    A hint: lets the kernels skip the index loads of absent offsets */
     int32_t        npass;       /* 1 or 2 */
     lb2_conv_io    io[2];
-    const int32_t* tile_order128;  /* from lb2_tile_order or NULL (tiles in row-order sequence, heaviest-looking last) */
-    const int32_t* tile_order256;
+    const int32_t* tile_order128;  /* from lb2_tile_order for this nbr / row_perm / d_mout, cdiv(mout_cap, 128) entries, or NULL (tiles
+                                      in row-order sequence).  Dispatch order of the tensor-core kernel's tiles (heaviest first);
+                                      ignored when nbr is NULL.  Scheduling only: results do not depend on it */
+    const int32_t* tile_order256;  /* not read by this build */
 } lb2_conv_desc;
 
 #define LB2_ALGO_AUTO  0

@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_scatter(const Params p) {
         cnt = min(BM, s_koff[k + 1] - pbase);
     };
 
-    if (warp < 4) {
+    if (warpgroup_role() == 0) {
         // =========================== producers ===========================
         const int sub = threadIdx.x & 7, rbase = threadIdx.x >> 3;
         // cp.async lookahead: stages still landing while the next is issued.  S - 2, not S - 1: a consumer releases a stage only once it

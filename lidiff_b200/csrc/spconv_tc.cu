@@ -6,13 +6,15 @@
 // three MMAs and is far less accurate.  Weights are pre-scaled by a power of two per layer so their low
 // parts stay in fp16's normal range; activations saturate at +-65504.)
 //
-// One CTA owns 128 output rows x NC output channels (NC = Cout, or Cout / 2 for Cout > 128: blockIdx.z picks
-// the half).  Warp roles (384 threads, three warpgroups):
+// One CTA owns 128 output rows x NC output channels of one guidance pass (NC = Cout, or Cout / 2 for Cout > 128).
+// blockIdx.x enumerates (tile slot, pass, channel half), the half fastest; slot i runs tile tile_order[i] (most
+// expensive first) when the map has a tile order.  Warp roles (384 threads, three warpgroups):
 //   warpgroup 0  producers: gather the neighbour rows of kernel offset k / channel chunk c (fp32 rows split to
 //                fp16 hi/lo in registers, or the fp16 split companions with cp.async) into the K-major
 //                SWIZZLE_128B shared-memory image; thread 0 also streams the pre-packed weight tiles of (k, c)
 //                with cp.async.bulk (mbarrier complete_tx).
-//   warpgroups 1, 2  consumers: rows [0, 64) / [64, 128) of the tile, 3 x (chunk / 16) wgmma per stage.
+//                Runs on 88 registers per thread (setmaxnreg) so that the consumers can take 208.
+//   warpgroups 1, 2  consumers: rows [0, 64) / [64, 128) of the tile, 3 x (chunk / 16) wgmma m64nNCk16 per stage.
 //                TWO-LEVEL ACCUMULATION: a long chain of tensor-core accumulations loses accuracy linearly with
 //                its length, so the chain is cut into groups of <= STEP_BUDGET MMA steps, each started from zero;
 //                after each group the partial sum is added to a running fp32 total in registers (round-to-nearest).
@@ -46,18 +48,33 @@ struct Params {
     const int* d_mout;
     int mout_cap;
     const int* row_perm;
+    const int* tile_order;                              // tile of dispatch slot i, -1 = no live tile; NULL = natural order
     int stages, nchunks, group;                         // group: kernel offsets per accumulation group
+    int npass, nsplit;
     lb2_conv_io io[2];
 };
+
+// Registers per thread after the producer warpgroup hands its surplus to the consumers.  The CTA is launched with 168 per thread
+// (65536 / 384, rounded down to the allocation granule of 8); 128 * PRODUCER_REGS + 256 * CONSUMER_REGS must stay within 384 * 168.
+// A consumer of NC = 128 holds 64 accumulator and 64 total registers; a producer of the fp32 path 16 float4 rows in flight.
+constexpr int PRODUCER_REGS = 88;
+constexpr int CONSUMER_REGS = 208;
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= THREADS * 168, "register split exceeds the CTA's allocation");
 
 template <int NC>
 __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
     extern __shared__ unsigned char smem_raw[];
     const int M = p.d_mout ? min(*p.d_mout, p.mout_cap) : p.mout_cap;
-    const int m0 = blockIdx.x * BM;
-    if (m0 >= M) return;
-    const lb2_conv_io io = p.io[blockIdx.y];
-    const int n0 = blockIdx.z * NC;                  // first output channel of this CTA
+    // blockIdx.x = (slot * npass + pass) * nsplit + half: the passes and channel halves of a tile run next to each other (their gathers
+    // of the same neighbour rows meet in L2), and slots follow the tile order, most expensive tile first, when there is one
+    const int half = blockIdx.x % p.nsplit;
+    const int pass = (blockIdx.x / p.nsplit) % p.npass;
+    const int slot_i = blockIdx.x / (p.nsplit * p.npass);
+    const int tile = p.tile_order ? __ldg(p.tile_order + slot_i) : slot_i;
+    const int m0 = tile * BM;
+    if (tile < 0 || m0 >= M) return;
+    const lb2_conv_io io = p.io[pass];
+    const int n0 = half * NC;                        // first output channel of this CTA
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ctot = p.c1 + p.c2;
 
@@ -113,8 +130,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
     const uint32_t kmask = misc[1];
     const int n_off = __popc(kmask);
 
-    if (warp < 4) {
+    if (warpgroup_role() == 0) {
         // =========================== producers: A gather (all 128 threads), B weights (thread 0) ===========================
+        setmaxnreg_dec<PRODUCER_REGS>();
         const int sub = threadIdx.x & 7;           // 8-channel group inside the 64-channel chunk
         const int rbase = threadIdx.x >> 3;        // 0..15
         const bool use_h = (io.in1_h != nullptr) && (p.c2 == 0 || io.in2_h != nullptr);   // fp16 split inputs: cp.async gather
@@ -169,39 +187,45 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
         }
     } else {
         // =========================== consumers: wgmma + two-level accumulation ===========================
+        setmaxnreg_inc<CONSUMER_REGS>();
         const int wg = (warp >> 2) - 1;                           // 0: tile rows [0, 64), 1: rows [64, 128)
+        // tot starts at -0: -0 + x == x for every x (+0 and -0 included), so the first fold is an exact copy without a select
         float acc[NC / 2], tot[NC / 2];
 #pragma unroll
-        for (int i = 0; i < NC / 2; ++i) tot[i] = 0.f;
-        int it = 0, in_group = 0, off_idx = 0, prev_s = -1;
-        bool have_tot = false;
-        for (uint32_t km = kmask; km; km &= km - 1, ++off_idx) {
-            for (int c = 0; c < p.nchunks; ++c, ++it) {
-                const int s = it % p.stages;
-                const uint32_t par = (it / p.stages) & 1;
-                mbar_wait(full_b(s), par);
-                mbar_wait(full_a(s), par);
-                const uint32_t a_hi = base + (uint32_t)s * stage_bytes + (uint32_t)wg * (A_TILE / 2), a_lo = a_hi + A_TILE;
-                const uint32_t b_hi = base + (uint32_t)s * stage_bytes + 2u * A_TILE, b_lo = b_hi + b_tile;
-                const int ksteps = min(KC, ctot - c * KC) >> 4;
-                reg_fence(acc);
-                wg_stage_mma<NC>(acc, a_hi, a_lo, b_hi, b_lo, ksteps, in_group == 0 && c == 0);   // first MMA of a group overwrites
-                reg_fence(acc);
-                wgmma_wait<1>();                                  // the MMAs of the previous stage are done: release it
-                if (prev_s >= 0 && lane == 0) mbar_arrive(empty(prev_s));
-                prev_s = s;
-            }
-            if (++in_group == p.group || off_idx == n_off - 1) {  // partial sum of this group complete -> running total
+        for (int i = 0; i < NC / 2; ++i) tot[i] = -0.f;
+        // one flat loop over the stages (offset-major, chunk-minor), the stage sequence the producers publish
+        const int n_it = n_off * p.nchunks;
+        int c = 0, in_group = 0, off_idx = 0, prev_s = -1;
+        for (int it = 0; it < n_it; ++it) {
+            const int s = it % p.stages;
+            const uint32_t par = (it / p.stages) & 1;
+            mbar_wait(full_b(s), par);
+            mbar_wait(full_a(s), par);
+            const uint32_t a_hi = base + (uint32_t)s * stage_bytes + (uint32_t)wg * (A_TILE / 2), a_lo = a_hi + A_TILE;
+            const uint32_t b_hi = base + (uint32_t)s * stage_bytes + 2u * A_TILE, b_lo = b_hi + b_tile;
+            const int ksteps = min(KC, ctot - c * KC) >> 4;
+            reg_fence(acc);
+            wg_stage_mma<NC>(acc, a_hi, a_lo, b_hi, b_lo, ksteps, in_group == 0 && c == 0);   // first MMA of a group overwrites
+            reg_fence(acc);
+            wgmma_wait<1>();                                      // the MMAs of the previous stage are done: release it
+            if (prev_s >= 0 && lane == 0) mbar_arrive(empty(prev_s));
+            prev_s = s;
+            if (++c < p.nchunks) continue;
+            c = 0;
+            ++off_idx;
+            if (++in_group == p.group || off_idx == n_off) {      // partial sum of this group complete -> running total
                 wgmma_wait<0>();
                 reg_fence(acc);
                 if (lane == 0) mbar_arrive(empty(prev_s));
                 prev_s = -1;
 #pragma unroll
-                for (int i = 0; i < NC / 2; ++i) tot[i] = have_tot ? __fadd_rn(tot[i], acc[i]) : acc[i];
-                have_tot = true;
+                for (int i = 0; i < NC / 2; ++i) tot[i] = __fadd_rn(tot[i], acc[i]);
                 in_group = 0;
             }
         }
+        // the last stage always ends a group, so nothing is in flight here; ptxas cannot see that, and without this wait it injects one
+        // on the loop's exit edge (C7517) before the epilogue reuses the accumulator registers
+        wgmma_wait<0>();
         // ---- totals -> shared-memory staging tile (the stage ring is idle once both consumer warpgroups are here) ----------
         const float out_scale = __ldg(reinterpret_cast<const float*>(p.wpacked) + 1);     // 2^-k of the packed weights
         float* stage_c = reinterpret_cast<float*>(gen);            // [BM][pitch] fp32
@@ -317,12 +341,11 @@ static size_t smem_bytes(int nc, int stages) {
 }
 
 template <int NC>
-static int launch(Lb2Handle* h, cudaStream_t s, const Params& p, int npass, int nsplit, int stages) {
+static int launch(Lb2Handle* h, cudaStream_t s, const Params& p, int stages) {
     const size_t smem = smem_bytes(NC, stages);
     cudaError_t e = lb2_configure_smem(h, LB2_K_TC + (NC / 32 - 1), k_spconv_tc<NC>, (int)(227 * 1024));
     if (e != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "k_spconv_tc smem attribute: %s", cudaGetErrorString(e));
-    dim3 grid(cdiv(p.mout_cap, BM), npass, nsplit);
-    k_spconv_tc<NC><<<grid, THREADS, smem, s>>>(p);
+    k_spconv_tc<NC><<<cdiv(p.mout_cap, BM) * p.npass * p.nsplit, THREADS, smem, s>>>(p);
     LB2_POST_LAUNCH(h, "k_spconv_tc");
     return LB2_OK;
 }
@@ -358,10 +381,13 @@ int lb2_spconv_tc_launch(Lb2Handle* h, cudaStream_t s, const lb2_conv_desc* d) {
     p.wpacked = (const unsigned char*)d->weight_packed;
     p.scale = d->scale; p.shift = d->shift; p.relu = d->relu;
     p.nbr = d->nbr; p.nbr_stride = d->nbr_stride; p.d_mout = d->d_mout; p.mout_cap = d->mout_cap; p.row_perm = d->row_perm;
+    p.tile_order = d->nbr ? d->tile_order128 : nullptr;     // the tile order ranks the tiles of a map's row order
     p.nchunks = (d->c1 + d->c2 + tc::KC - 1) / tc::KC;
     // a consumer thread holds NC / 2 accumulator and NC / 2 total registers: NC <= 128, so Cout 256 runs as two CTAs of 128 channels
     const int nsplit = d->cout > 128 ? 2 : 1;
     const int nc = d->cout / nsplit;
+    p.npass = d->npass > 1 ? 2 : 1;
+    p.nsplit = nsplit;
     int stages = tc::MAX_STAGES;
     while (stages > 2 && tc::smem_bytes(nc, stages) > 227 * 1024) --stages;
     p.stages = stages;
@@ -369,10 +395,10 @@ int lb2_spconv_tc_launch(Lb2Handle* h, cudaStream_t s, const lb2_conv_desc* d) {
     p.group = std::max(1, tc::STEP_BUDGET / steps_per_offset);
     p.io[0] = d->io[0]; p.io[1] = d->io[d->npass > 1 ? 1 : 0];
     switch (nc) {
-        case 32: return tc::launch<32>(h, s, p, d->npass, nsplit, stages);
-        case 64: return tc::launch<64>(h, s, p, d->npass, nsplit, stages);
-        case 96: return tc::launch<96>(h, s, p, d->npass, nsplit, stages);
-        case 128: return tc::launch<128>(h, s, p, d->npass, nsplit, stages);
+        case 32: return tc::launch<32>(h, s, p, stages);
+        case 64: return tc::launch<64>(h, s, p, stages);
+        case 96: return tc::launch<96>(h, s, p, stages);
+        case 128: return tc::launch<128>(h, s, p, stages);
         default: return lb2_fail(h, LB2_ERR_UNSUP, "tensor-core variant: no kernel for %s output channels per CTA", nc == 80 ? "80" : nc == 112 ? "112" : "this many");
     }
 }

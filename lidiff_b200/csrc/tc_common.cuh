@@ -53,12 +53,6 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 // D(64 x n, fp32 registers) (+)= A(64 x 16, smem) . B(n x 16, smem)^T, both operands fp16 K-major.  accumulate = 0 overwrites D.
 // Register i of the calling thread (warp w, lane l of the warpgroup) holds row 16 w + l / 4 + 8 ((i / 2) & 1),
 // column 8 (i / 4) + 2 (l % 4) + (i & 1).
-__device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "l"(da), "l"(db), "r"(accumulate) : "memory");
-}
 __device__ __forceinline__ void wgmma_m64n32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
@@ -75,35 +69,76 @@ __device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t da, uint64_t db,
           "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-
-// D(64 x N) for N a multiple of 16: n64 / n32 / n16 instructions side by side, B rows (= output channels) advance 128 bytes each
-template <int N, int OFF = 0>
-__device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint32_t b_addr, uint32_t accumulate) {
-    constexpr int REST = N - OFF;
-    if constexpr (REST >= 64) {
-        wgmma_m64n64(d + OFF / 2, da, make_desc(b_addr + OFF * 128), accumulate);
-        wgmma_n<N, OFF + 64>(d, da, b_addr, accumulate);
-    } else if constexpr (REST >= 32) {
-        wgmma_m64n32(d + OFF / 2, da, make_desc(b_addr + OFF * 128), accumulate);
-        wgmma_n<N, OFF + 32>(d, da, b_addr, accumulate);
-    } else if constexpr (REST >= 16) {
-        wgmma_m64n16(d + OFF / 2, da, make_desc(b_addr + OFF * 128), accumulate);
-    }
+__device__ __forceinline__ void wgmma_m64n96(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-// one pipeline stage of the FP16x3 product for the calling warpgroup: rows [64 wg, +64) of the A tiles (hi, lo) times the N rows of
-// the B tiles (hi, lo), ksteps 16-channel steps, 3 MMAs each (x_hi.w_hi + x_lo.w_hi + x_hi.w_lo); first = overwrite D
+__device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+
+// D(64 x N) for N = 32 / 64 / 96 / 128 as ONE instruction: every B row (= output channel) of the tile in one MMA, so each A slice is
+// read from shared memory once per (A, B) pair.  The register layout above holds for any N, so D is the same array as before.
 template <int N>
-__device__ __forceinline__ void wg_stage_mma(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int ksteps, bool first) {
-    wgmma_fence();
-#pragma unroll 1
-    for (int ks = 0; ks < ksteps; ++ks) {
+__device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64 || N == 96 || N == 128, "wgmma_n: N must be 32, 64, 96 or 128");
+    if constexpr (N == 128) wgmma_m64n128(d, da, db, accumulate);
+    else if constexpr (N == 96) wgmma_m64n96(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_m64n64(d, da, db, accumulate);
+    else wgmma_m64n32(d, da, db, accumulate);
+}
+template <int N, int KSTEPS>
+__device__ __forceinline__ void wg_stage_mma_k(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, uint32_t acc0) {
+    wgmma_fence();          // in the MMAs' own basic block: a fence behind a branch makes ptxas inject warpgroup.arrive (C7519)
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks) {
         const uint64_t dah = make_desc(a_hi + ks * 32), dal = make_desc(a_lo + ks * 32);
-        wgmma_n<N>(d, dah, b_hi + ks * 32, (first && ks == 0) ? 0u : 1u);
-        wgmma_n<N>(d, dal, b_hi + ks * 32, 1u);
-        wgmma_n<N>(d, dah, b_lo + ks * 32, 1u);
+        const uint64_t dbh = make_desc(b_hi + ks * 32), dbl = make_desc(b_lo + ks * 32);
+        wgmma_n<N>(d, dah, dbh, ks == 0 ? acc0 : 1u);
+        wgmma_n<N>(d, dal, dbh, 1u);
+        wgmma_n<N>(d, dah, dbl, 1u);
     }
     wgmma_commit();
 }
+// one pipeline stage of the FP16x3 product for the calling warpgroup: rows [64 wg, +64) of the A tiles (hi, lo) times the N rows of
+// the B tiles (hi, lo), ksteps 16-channel steps, 3 MMAs each (x_hi.w_hi + x_lo.w_hi + x_hi.w_lo); first = overwrite D.
+// ksteps is 4 except in the last chunk of a channel count that is not a multiple of 64 (channel counts are multiples of 16): every
+// case is a fully unrolled instruction sequence, so no loop counter or accumulator copy sits between the MMAs of a stage.
+template <int N>
+__device__ __forceinline__ void wg_stage_mma(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int ksteps, bool first) {
+    const uint32_t acc0 = first ? 0u : 1u;
+    if (ksteps == 4) wg_stage_mma_k<N, 4>(d, a_hi, a_lo, b_hi, b_lo, acc0);
+    else if (ksteps == 2) wg_stage_mma_k<N, 2>(d, a_hi, a_lo, b_hi, b_lo, acc0);
+    else if (ksteps == 1) wg_stage_mma_k<N, 1>(d, a_hi, a_lo, b_hi, b_lo, acc0);
+    else wg_stage_mma_k<N, 3>(d, a_hi, a_lo, b_hi, b_lo, acc0);
+}
+// role of the calling thread's warpgroup (threadIdx.x / 128), read from lane 0 so that the compiler sees a warp-uniform value: a
+// branch on threadIdx.x itself counts as divergent, and ptxas then serialises every wgmma behind it (C7520)
+__device__ __forceinline__ int warpgroup_role() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0); }
+// hand registers from the producer warpgroup to the consumer warpgroups (the CTA's register file is fixed at launch)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
 __device__ __forceinline__ void reg_fence(float (&d)[R]) {      // keeps the compiler from moving accumulator accesses across a wgmma wait
 #pragma unroll
