@@ -163,7 +163,8 @@ typedef struct {
     int32_t        mout_cap;
     const int32_t* row_perm;    /* execution order from lb2_row_order or NULL (natural order) */
     const uint32_t* row_mask;   /* per output row: bit k set <=> nbr[k][row] >= 0 (lb2_kernel_map's row_mask) or NULL.
-                                   A hint: lets the kernels skip the index loads of absent offsets */
+                                   Lets the kernels skip the index loads of absent offsets: the tensor-core kernel loads only
+                                   the offsets whose bit is set, so a mask must not miss an entry of nbr */
     int32_t        npass;       /* 1 or 2 */
     lb2_conv_io    io[2];
     const int32_t* tile_order128;  /* from lb2_tile_order for this nbr / row_perm / d_mout, cdiv(mout_cap, 128) entries, or NULL (tiles

@@ -48,6 +48,7 @@ struct Params {
     const int* d_mout;
     int mout_cap;
     const int* row_perm;
+    const unsigned* row_mask;                           // per output row: bit k <=> nbr[k][row] >= 0; NULL = load every offset
     const int* tile_order;                              // tile of dispatch slot i, -1 = no live tile; NULL = natural order
     int stages, nchunks, group;                         // group: kernel offsets per accumulation group
     int npass, nsplit;
@@ -106,24 +107,24 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
         const int slot = m0 + threadIdx.x;
         const int row = (slot < M) ? (p.row_perm ? __ldg(p.row_perm + slot) : slot) : -1;
         row_s[threadIdx.x] = row;
-        uint32_t mymask = 0;
-        for (int k0 = 0; k0 < p.kvol; k0 += 9) {        // 9 independent loads in flight, then the votes
-            int v[9];
+        // the row's neighbour mask names the offsets that have an entry: only those index loads are issued, all at once (the sparse
+        // levels' rows have a few of 27, and the loads hit random rows of the map).  Without a mask every offset is loaded.
+        const uint32_t want = row < 0 ? 0u : (p.row_mask ? __ldg(p.row_mask + row) : ~0u);
+        int v[MAX_KVOL];
 #pragma unroll
-            for (int q = 0; q < 9; ++q) {
-                const int k = k0 + q;
-                v[q] = -1;
-                if (k < p.kvol && row >= 0) v[q] = p.nbr ? __ldg(p.nbr + (long long)k * p.nbr_stride + row) : row;
-            }
+        for (int k = 0; k < MAX_KVOL; ++k) {
+            v[k] = -1;
+            if (k < p.kvol && ((want >> k) & 1u)) v[k] = p.nbr ? __ldg(p.nbr + (long long)k * p.nbr_stride + row) : row;
+        }
+        uint32_t have = 0;
 #pragma unroll
-            for (int q = 0; q < 9; ++q) {
-                const int k = k0 + q;
-                if (k < p.kvol) {
-                    idx_s[k * BM + threadIdx.x] = v[q];
-                    if (__any_sync(0xffffffffu, v[q] >= 0)) mymask |= 1u << k;
-                }
+        for (int k = 0; k < MAX_KVOL; ++k) {
+            if (k < p.kvol) {
+                idx_s[k * BM + threadIdx.x] = v[k];
+                if (v[k] >= 0) have |= 1u << k;
             }
         }
+        const uint32_t mymask = __reduce_or_sync(0xffffffffu, have);
         if (lane == 0 && mymask) atomicOr(&misc[1], mymask);
     }
     __syncthreads();
@@ -382,6 +383,7 @@ int lb2_spconv_tc_launch(Lb2Handle* h, cudaStream_t s, const lb2_conv_desc* d) {
     p.scale = d->scale; p.shift = d->shift; p.relu = d->relu;
     p.nbr = d->nbr; p.nbr_stride = d->nbr_stride; p.d_mout = d->d_mout; p.mout_cap = d->mout_cap; p.row_perm = d->row_perm;
     p.tile_order = d->nbr ? d->tile_order128 : nullptr;     // the tile order ranks the tiles of a map's row order
+    p.row_mask = d->nbr ? (const unsigned*)d->row_mask : nullptr;
     p.nchunks = (d->c1 + d->c2 + tc::KC - 1) / tc::KC;
     // a consumer thread holds NC / 2 accumulator and NC / 2 total registers: NC <= 128, so Cout 256 runs as two CTAs of 128 channels
     const int nsplit = d->cout > 128 ? 2 : 1;
