@@ -115,8 +115,8 @@ int lb2_row_order(void* h, void* stream, const uint32_t* row_mask, const int32_t
 /* Cost order of the tiles of a map (scheduling only; results do not depend on it): order128[i] / order256[i] = index of the i-th most
  * expensive 128-row tile / 256-row super-tile of the row order `row_perm`, cost = number of kernel offsets the tile has to run (popcount of
  * the OR of its rows' masks); entries beyond the live tile count are -1.  The tensor-core convolution (lb2_conv_desc.tile_order128)
- * launches its tiles in this order, most expensive first, so that the cheap tiles fill the tail of the launch; order256 is for a
- * kernel that deals 256-row super-tiles to persistent CTAs and is not read by this build.
+ * deals its tiles to its persistent CTAs in this order, most expensive first, so that the cheap tiles fill the end of the launch;
+ * order256 (256-row super-tiles) is not read by this build.
  * order128: cdiv(n_cap,128) ints, order256: cdiv(n_cap,256) ints, scratch: cdiv(n_cap,128) * 4 bytes. */
 int lb2_tile_order(void* h, void* stream, const uint32_t* row_mask, const int32_t* row_perm, const int32_t* d_n, int32_t n_cap,
                    int32_t* order128, int32_t* order256, void* scratch);
@@ -168,15 +168,16 @@ typedef struct {
     int32_t        npass;       /* 1 or 2 */
     lb2_conv_io    io[2];
     const int32_t* tile_order128;  /* from lb2_tile_order for this nbr / row_perm / d_mout, cdiv(mout_cap, 128) entries, or NULL (tiles
-                                      in row-order sequence).  Dispatch order of the tensor-core kernel's tiles (heaviest first);
-                                      ignored when nbr is NULL.  Scheduling only: results do not depend on it */
+                                      in row-order sequence).  Order in which the tensor-core kernel deals its tiles to its
+                                      persistent CTAs (heaviest first); ignored when nbr is NULL.  Scheduling only: results do not
+                                      depend on it */
     const int32_t* tile_order256;  /* not read by this build */
 } lb2_conv_desc;
 
 #define LB2_ALGO_AUTO  0
 #define LB2_ALGO_FFMA  1    /* fp32 CUDA-core implicit GEMM */
-#define LB2_ALGO_TC    2    /* wgmma FP16x3 split-precision implicit GEMM (needs weight_packed), one CTA per 128-row tile */
-#define LB2_ALGO_TC_TILE 3  /* the same kernel (kept as an alias: callers that name the per-tile form) */
+#define LB2_ALGO_TC    2    /* wgmma FP16x3 split-precision implicit GEMM (needs weight_packed), persistent CTAs over 128-row tiles */
+#define LB2_ALGO_TC_TILE 3  /* the same kernel (an alias kept for callers that name it) */
 int lb2_spconv_forward(void* h, void* stream, const lb2_conv_desc* d, int algo);
 
 /* The same convolution in gather-GEMM-scatter form (what ME's GPU backend does per kernel offset) for levels

@@ -6,19 +6,24 @@
 // three MMAs and is far less accurate.  Weights are pre-scaled by a power of two per layer so their low
 // parts stay in fp16's normal range; activations saturate at +-65504.)
 //
-// One CTA owns 128 output rows x NC output channels of one guidance pass (NC = Cout, or Cout / 2 for Cout > 128).
-// blockIdx.x enumerates (tile slot, pass, channel half), the half fastest; slot i runs tile tile_order[i] (most
-// expensive first) when the map has a tile order.  Warp roles (384 threads, three warpgroups):
-//   warpgroup 0  producers: gather the neighbour rows of kernel offset k / channel chunk c (fp32 rows split to
+// A work item is 128 output rows x NC output channels of one guidance pass (NC = Cout, or Cout / 2 for Cout > 128).
+// Items are numbered (tile slot, pass, channel half), the half fastest; slot i is tile tile_order[i] (most expensive
+// first) when the map has a tile order.  The kernel is persistent: one CTA per SM, CTA b runs items b, b + G, b + 2G, ...
+// (G = grid size) and stops at its first item past the live tiles.  The stage ring runs across items: the producers
+// gather the next tile while the consumers finish the current one and run its epilogue.  Warp roles (384 threads):
+//   warpgroup 0  producers: per item, first the tile's index table (one thread per row: output row, neighbour indices
+//                of the offsets its row mask names, OR of the tile's offset mask) into one of two tile-info buffers;
+//                then gather the neighbour rows of kernel offset k / channel chunk c (fp32 rows split to
 //                fp16 hi/lo in registers, or the fp16 split companions with cp.async) into the K-major
 //                SWIZZLE_128B shared-memory image; thread 0 also streams the pre-packed weight tiles of (k, c)
-//                with cp.async.bulk (mbarrier complete_tx).
+//                with cp.async.bulk (mbarrier complete_tx).  After a tile's last stage they publish one more ring
+//                slot without loads, the epilogue slot, in which the consumers stage the tile's totals.
 //                Runs on 88 registers per thread (setmaxnreg) so that the consumers can take 208.
 //   warpgroups 1, 2  consumers: rows [0, 64) / [64, 128) of the tile, 3 x (chunk / 16) wgmma m64nNCk16 per stage.
 //                TWO-LEVEL ACCUMULATION: a long chain of tensor-core accumulations loses accuracy linearly with
 //                its length, so the chain is cut into groups of <= STEP_BUDGET MMA steps, each started from zero;
 //                after each group the partial sum is added to a running fp32 total in registers (round-to-nearest).
-//                The totals go through a shared-memory staging tile to a coalesced epilogue:
+//                The totals go through the epilogue slot to a coalesced epilogue:
 //                BN affine + residual + ReLU + gate -> global.
 // Kernel offsets where none of the tile's 128 rows has a neighbour are skipped by every role.
 //
@@ -62,225 +67,283 @@ constexpr int PRODUCER_REGS = 88;
 constexpr int CONSUMER_REGS = 208;
 static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= THREADS * 168, "register split exceeds the CTA's allocation");
 
+// What the producers know of a work item and the consumers need: written by the producers' prologue, read by the producers' gather
+// (idx) and by the consumers (mask, item; row in the epilogue).  Two buffers, so that the next item's table is built while the
+// consumers still run the current one.
+struct TileInfo {
+    int idx[MAX_KVOL * BM];      // neighbour row of (kernel offset k, tile row r) at [k * BM + r], -1 = none
+    int row[BM];                 // output row of each tile row, -1 beyond the live rows
+    uint32_t mask[4];            // per producer warp: OR of its rows' offset masks
+    int item;                    // work item, -1 = this CTA has no more
+    int pad[3];
+};
+// dynamic shared memory: 1024-byte alignment slack | stage ring | two tile-info buffers | mbarriers
+constexpr int NUM_BARS = 3 * MAX_STAGES + 4;
+
 template <int NC>
 __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
     extern __shared__ unsigned char smem_raw[];
     const int M = p.d_mout ? min(*p.d_mout, p.mout_cap) : p.mout_cap;
-    // blockIdx.x = (slot * npass + pass) * nsplit + half: the passes and channel halves of a tile run next to each other (their gathers
-    // of the same neighbour rows meet in L2), and slots follow the tile order, most expensive tile first, when there is one
-    const int half = blockIdx.x % p.nsplit;
-    const int pass = (blockIdx.x / p.nsplit) % p.npass;
-    const int slot_i = blockIdx.x / (p.nsplit * p.npass);
-    const int tile = p.tile_order ? __ldg(p.tile_order + slot_i) : slot_i;
-    const int m0 = tile * BM;
-    if (tile < 0 || m0 >= M) return;
-    const lb2_conv_io io = p.io[pass];
-    const int n0 = half * NC;                        // first output channel of this CTA
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ctot = p.c1 + p.c2;
+    const int S = p.stages;
 
     // ---- shared memory carve-up (tiles 1024-byte aligned for SWIZZLE_128B) -----------------------------
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     unsigned char* gen = smem_raw + (base - raw);
-    constexpr uint32_t b_tile = (uint32_t)NC * 128u;                 // one fp16 B tile (hi or lo) of this CTA's channels
+    constexpr uint32_t b_tile = (uint32_t)NC * 128u;                 // one fp16 B tile (hi or lo) of an item's channels
     const uint32_t b_full = (uint32_t)p.cout * 128u;                 // the same tile over all cout channels (packed layout)
     const uint32_t stage_bytes = 2u * A_TILE + 2u * b_tile;
-    unsigned char* tail = gen + (size_t)p.stages * stage_bytes;
-    int* idx_s = reinterpret_cast<int*>(tail);                       // [kvol][BM]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(tail + MAX_KVOL * BM * sizeof(int));
-    uint32_t* misc = reinterpret_cast<uint32_t*>(bars + 3 * MAX_STAGES);      // [1] offset mask
-    int* row_s = reinterpret_cast<int*>(misc + 4);                             // [BM] output row of each tile slot
-    const uint32_t bar0 = smem_u32(bars);
+    TileInfo* info = reinterpret_cast<TileInfo*>(gen + (size_t)S * stage_bytes);
+    const uint32_t bar0 = smem_u32(info + 2);
     auto full_a = [&](int s) { return bar0 + 8u * s; };
     auto full_b = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
     auto empty = [&](int s) { return bar0 + 8u * (2 * MAX_STAGES + s); };
+    auto info_full = [&](int b) { return bar0 + 8u * (3 * MAX_STAGES + b); };
+    auto info_empty = [&](int b) { return bar0 + 8u * (3 * MAX_STAGES + 2 + b); };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.stages; ++s) { mbar_init(full_a(s), NUM_PRODUCER); mbar_init(full_b(s), 1); mbar_init(empty(s), NUM_CONSUMER_WARPS); }
-        misc[1] = 0;
+        for (int s = 0; s < S; ++s) { mbar_init(full_a(s), NUM_PRODUCER); mbar_init(full_b(s), 1); mbar_init(empty(s), NUM_CONSUMER_WARPS); }
+        for (int b = 0; b < 2; ++b) { mbar_init(info_full(b), NUM_PRODUCER); mbar_init(info_empty(b), NUM_CONSUMER_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    // ---- neighbour indices of this tile + mask of non-empty kernel offsets -----------------------------
-    if (threadIdx.x < BM) {
-        const int slot = m0 + threadIdx.x;
-        const int row = (slot < M) ? (p.row_perm ? __ldg(p.row_perm + slot) : slot) : -1;
-        row_s[threadIdx.x] = row;
-        // the row's neighbour mask names the offsets that have an entry: only those index loads are issued, all at once (the sparse
-        // levels' rows have a few of 27, and the loads hit random rows of the map).  Without a mask every offset is loaded.
-        const uint32_t want = row < 0 ? 0u : (p.row_mask ? __ldg(p.row_mask + row) : ~0u);
-        int v[MAX_KVOL];
-#pragma unroll
-        for (int k = 0; k < MAX_KVOL; ++k) {
-            v[k] = -1;
-            if (k < p.kvol && ((want >> k) & 1u)) v[k] = p.nbr ? __ldg(p.nbr + (long long)k * p.nbr_stride + row) : row;
-        }
-        uint32_t have = 0;
-#pragma unroll
-        for (int k = 0; k < MAX_KVOL; ++k) {
-            if (k < p.kvol) {
-                idx_s[k * BM + threadIdx.x] = v[k];
-                if (v[k] >= 0) have |= 1u << k;
-            }
-        }
-        const uint32_t mymask = __reduce_or_sync(0xffffffffu, have);
-        if (lane == 0 && mymask) atomicOr(&misc[1], mymask);
-    }
-    __syncthreads();
-    const uint32_t kmask = misc[1];
-    const int n_off = __popc(kmask);
 
+    // Ring slot `it` (data stage or epilogue slot) is ring stage it % S in phase it / S; both roles count it across items.  Item j of
+    // this CTA uses tile-info buffer j & 1 in phase j >> 1.
     if (warpgroup_role() == 0) {
-        // =========================== producers: A gather (all 128 threads), B weights (thread 0) ===========================
+        // =========================== producers: tile table, A gather (all 128 threads), B weights (thread 0) ===========================
         setmaxnreg_dec<PRODUCER_REGS>();
         const int sub = threadIdx.x & 7;           // 8-channel group inside the 64-channel chunk
         const int rbase = threadIdx.x >> 3;        // 0..15
-        const bool use_h = (io.in1_h != nullptr) && (p.c2 == 0 || io.in2_h != nullptr);   // fp16 split inputs: cp.async gather
         // cp.async lookahead: stages still landing while the next is issued.  S - 2, not S - 1: a consumer releases a stage only once it
         // holds the next one (wgmma_wait<1>), so the producers must be able to publish stage i + 1 while stage i - 1 is still held
-        const int D = max(p.stages - 2, 0);
+        const int D = max(S - 2, 0);
         int it = 0, arrived = 0;
-        for (uint32_t km = kmask; km; km &= km - 1) {
-            const int k = __ffs(km) - 1;
-            const int* idxk = idx_s + k * BM;
-            int src[8];
+        // item x = (slot * npass + pass) * nsplit + half: the passes and channel halves of a tile are consecutive items and run on
+        // neighbouring CTAs at the same time (their gathers of the same neighbour rows meet in L2); slots follow the tile order, most
+        // expensive tile first, when there is one, so the static stride deals the tiles roughly longest first
+        auto tile_of = [&](int x) {
+            const int slot_i = x / (p.nsplit * p.npass);
+            return slot_i * BM >= p.mout_cap ? -1 : p.tile_order ? __ldg(p.tile_order + slot_i) : slot_i;
+        };
+        // index loads of tile row threadIdx.x: its output row and the neighbour row of every kernel offset (-1 = none).  The row's
+        // neighbour mask names the offsets that have an entry: only those index loads are issued, all at once (the sparse levels' rows
+        // have a few of 27, and the loads hit random rows of the map).  Without a mask every offset is loaded.
+        auto load_row = [&](int tile) {
+            const int slot = tile * BM + threadIdx.x;
+            return (tile >= 0 && slot < M) ? (p.row_perm ? __ldg(p.row_perm + slot) : slot) : -1;
+        };
+        auto load_indices = [&](int row, int (&v)[MAX_KVOL]) {
+            const uint32_t want = row < 0 ? 0u : (p.row_mask ? __ldg(p.row_mask + row) : ~0u);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) src[j] = idxk[rbase + 16 * j];
-            for (int c = 0; c < p.nchunks; ++c, ++it) {
-                const int s = it % p.stages;
-                mbar_wait(empty(s), ((it / p.stages) & 1) ^ 1);
-                unsigned char* a_hi = gen + (size_t)s * stage_bytes;
-                const uint32_t a_hi_u = base + (uint32_t)s * stage_bytes;
-                if (threadIdx.x == 0) {
-                    const uint32_t dst = a_hi_u + 2u * A_TILE;
-                    const unsigned char* wsrc = p.wpacked + PACK_HEADER + ((size_t)k * p.nchunks + c) * (2u * b_full) + (size_t)n0 * 128u;
-                    mbar_expect_tx(full_b(s), 2u * b_tile);
-                    bulk_g2s(dst, wsrc, b_tile, full_b(s));                      // hi rows n0 .. n0+NC
-                    bulk_g2s(dst + b_tile, wsrc + b_full, b_tile, full_b(s));    // lo rows
+            for (int k = 0; k < MAX_KVOL; ++k) {
+                v[k] = -1;
+                if (k < p.kvol && ((want >> k) & 1u)) v[k] = p.nbr ? __ldg(p.nbr + (long long)k * p.nbr_stride + row) : row;
+            }
+        };
+        int x = blockIdx.x, tile = tile_of(x), row = load_row(tile), v[MAX_KVOL];
+        load_indices(row, v);
+        for (int j = 0;; ++j) {
+            TileInfo& ti = info[j & 1];
+            mbar_wait(info_empty(j & 1), ((j >> 1) & 1) ^ 1);
+            if (tile < 0 || tile * BM >= M) {      // the dead items are the last ones: this CTA is done
+                if (threadIdx.x == 0) ti.item = -1;
+                mbar_arrive(info_full(j & 1));
+                break;
+            }
+            // ---- the tile's index table + mask of non-empty kernel offsets: one thread per tile row ----
+            {
+                ti.row[threadIdx.x] = row;
+                uint32_t have = 0;
+#pragma unroll
+                for (int k = 0; k < MAX_KVOL; ++k) {
+                    if (k < p.kvol) {
+                        ti.idx[k * BM + threadIdx.x] = v[k];
+                        if (v[k] >= 0) have |= 1u << k;
+                    }
                 }
-                const int ch = c * KC + sub * 8;
-                if (ch < ctot) {
-                    const bool first = ch < p.c1;
-                    const int cw = first ? p.c1 : p.c2;
-                    const int co = first ? ch : ch - p.c1;
-                    if (use_h) produce_a_split(reinterpret_cast<const __half*>(first ? io.in1_h : io.in2_h), cw, co, src, a_hi_u, a_hi_u + A_TILE, rbase, sub);
-                    else produce_a_f32(first ? io.in1 : io.in2, cw, co, src, a_hi, a_hi + A_TILE, rbase, sub);
-                }
-                if (use_h) {
+                const uint32_t wmask = __reduce_or_sync(0xffffffffu, have);
+                if (lane == 0) ti.mask[warp] = wmask;
+                if (threadIdx.x == 0) ti.item = x;
+            }
+            mbar_arrive(info_full(j & 1));
+            mbar_wait(info_full(j & 1), (j >> 1) & 1);         // the other producer warps' rows and masks
+            const uint32_t kmask = ti.mask[0] | ti.mask[1] | ti.mask[2] | ti.mask[3];
+            const int x_next = x + gridDim.x;
+            const int tile_next = tile_of(x_next);              // loaded now, used after the tile's stages
+            const int n0 = (x % p.nsplit) * NC;                 // first output channel of the item
+            const lb2_conv_io io = p.io[(x / p.nsplit) % p.npass];
+            const bool use_h = (io.in1_h != nullptr) && (p.c2 == 0 || io.in2_h != nullptr);   // fp16 split inputs: cp.async gather
+            for (uint32_t km = kmask; km; km &= km - 1) {
+                const int k = __ffs(km) - 1;
+                const int* idxk = ti.idx + k * BM;
+                int src[8];
+#pragma unroll
+                for (int r = 0; r < 8; ++r) src[r] = idxk[rbase + 16 * r];
+                for (int c = 0; c < p.nchunks; ++c) {
+                    const int s = it % S;
+                    mbar_wait(empty(s), ((it / S) & 1) ^ 1);
+                    unsigned char* a_hi = gen + (size_t)s * stage_bytes;
+                    const uint32_t a_hi_u = base + (uint32_t)s * stage_bytes;
+                    if (threadIdx.x == 0) {
+                        const uint32_t dst = a_hi_u + 2u * A_TILE;
+                        const unsigned char* wsrc = p.wpacked + PACK_HEADER + ((size_t)k * p.nchunks + c) * (2u * b_full) + (size_t)n0 * 128u;
+                        mbar_expect_tx(full_b(s), 2u * b_tile);
+                        bulk_g2s(dst, wsrc, b_tile, full_b(s));                      // hi rows n0 .. n0+NC
+                        bulk_g2s(dst + b_tile, wsrc + b_full, b_tile, full_b(s));    // lo rows
+                    }
+                    const int ch = c * KC + sub * 8;
+                    if (ch < ctot) {
+                        const bool first = ch < p.c1;
+                        const int cw = first ? p.c1 : p.c2;
+                        const int co = first ? ch : ch - p.c1;
+                        if (use_h) produce_a_split(reinterpret_cast<const __half*>(first ? io.in1_h : io.in2_h), cw, co, src, a_hi_u, a_hi_u + A_TILE, rbase, sub);
+                        else produce_a_f32(first ? io.in1 : io.in2, cw, co, src, a_hi, a_hi + A_TILE, rbase, sub);
+                    }
+                    // one protocol for both paths (consecutive items may take different ones): a cp.async group per stage (empty for the
+                    // fp32 path), published D stages later
                     cp_async_commit();
-                    if (it >= D) {                 // the copies of iteration it-D have landed
+                    ++it;
+                    if (it - arrived > D) {
                         cp_async_wait_dyn(D);
                         fence_proxy_async();
-                        mbar_arrive(full_a(arrived % p.stages));
+                        mbar_arrive(full_a(arrived % S));
                         ++arrived;
                     }
-                } else {
-                    fence_proxy_async();
-                    mbar_arrive(full_a(s));
                 }
             }
-        }
-        if (use_h) {
+            // the epilogue slot: no loads, the consumers stage the tile's totals in it.  Then everything still owed is published, so
+            // neither the tile's last stages nor its epilogue wait for the next tile's index loads.
+            const int s = it % S;
+            mbar_wait(empty(s), ((it / S) & 1) ^ 1);
+            if (threadIdx.x == 0) mbar_arrive(full_b(s));
+            ++it;
+            x = x_next;
+            tile = tile_next;
+            row = load_row(tile);                  // in flight while the last stages land
             cp_async_wait<0>();
             fence_proxy_async();
-            for (; arrived < it; ++arrived) mbar_arrive(full_a(arrived % p.stages));
+            for (; arrived < it; ++arrived) mbar_arrive(full_a(arrived % S));
+            load_indices(row, v);
         }
     } else {
-        // =========================== consumers: wgmma + two-level accumulation ===========================
+        // =========================== consumers: wgmma + two-level accumulation, epilogue ===========================
         setmaxnreg_inc<CONSUMER_REGS>();
         const int wg = (warp >> 2) - 1;                           // 0: tile rows [0, 64), 1: rows [64, 128)
-        // tot starts at -0: -0 + x == x for every x (+0 and -0 included), so the first fold is an exact copy without a select
-        float acc[NC / 2], tot[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; ++i) tot[i] = -0.f;
-        // one flat loop over the stages (offset-major, chunk-minor), the stage sequence the producers publish
-        const int n_it = n_off * p.nchunks;
-        int c = 0, in_group = 0, off_idx = 0, prev_s = -1;
-        for (int it = 0; it < n_it; ++it) {
-            const int s = it % p.stages;
-            const uint32_t par = (it / p.stages) & 1;
-            mbar_wait(full_b(s), par);
-            mbar_wait(full_a(s), par);
-            const uint32_t a_hi = base + (uint32_t)s * stage_bytes + (uint32_t)wg * (A_TILE / 2), a_lo = a_hi + A_TILE;
-            const uint32_t b_hi = base + (uint32_t)s * stage_bytes + 2u * A_TILE, b_lo = b_hi + b_tile;
-            const int ksteps = min(KC, ctot - c * KC) >> 4;
-            reg_fence(acc);
-            wg_stage_mma<NC>(acc, a_hi, a_lo, b_hi, b_lo, ksteps, in_group == 0 && c == 0);   // first MMA of a group overwrites
-            reg_fence(acc);
-            wgmma_wait<1>();                                      // the MMAs of the previous stage are done: release it
-            if (prev_s >= 0 && lane == 0) mbar_arrive(empty(prev_s));
-            prev_s = s;
-            if (++c < p.nchunks) continue;
-            c = 0;
-            ++off_idx;
-            if (++in_group == p.group || off_idx == n_off) {      // partial sum of this group complete -> running total
-                wgmma_wait<0>();
-                reg_fence(acc);
-                if (lane == 0) mbar_arrive(empty(prev_s));
-                prev_s = -1;
-#pragma unroll
-                for (int i = 0; i < NC / 2; ++i) tot[i] = __fadd_rn(tot[i], acc[i]);
-                in_group = 0;
-            }
-        }
-        // the last stage always ends a group, so nothing is in flight here; ptxas cannot see that, and without this wait it injects one
-        // on the loop's exit edge (C7517) before the epilogue reuses the accumulator registers
-        wgmma_wait<0>();
-        // ---- totals -> shared-memory staging tile (the stage ring is idle once both consumer warpgroups are here) ----------
         const float out_scale = __ldg(reinterpret_cast<const float*>(p.wpacked) + 1);     // 2^-k of the packed weights
-        float* stage_c = reinterpret_cast<float*>(gen);            // [BM][pitch] fp32
-        constexpr int pitch = NC + 4;                              // +4 floats: fewer bank conflicts on the row reads
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        {
-            const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        int it = 0;
+        for (int j = 0;; ++j) {
+            const TileInfo& ti = info[j & 1];
+            mbar_wait(info_full(j & 1), (j >> 1) & 1);
+            const int x = ti.item;
+            if (x < 0) break;
+            const int n_off = __popc(ti.mask[0] | ti.mask[1] | ti.mask[2] | ti.mask[3]);
+            // tot starts at -0: -0 + x == x for every x (+0 and -0 included), so the first fold is an exact copy without a select
+            float acc[NC / 2], tot[NC / 2];
 #pragma unroll
-            for (int i = 0; i < NC / 2; i += 2) {
-                const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3);
-                *reinterpret_cast<float2*>(stage_c + row * pitch + col) = make_float2(tot[i] * out_scale, tot[i + 1] * out_scale);
-            }
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        // ---- epilogue, coalesced: consumer warp cw owns tile rows cw, cw + 8, ... and walks their (row, 4-channel) elements with
-        //      consecutive lanes on consecutive channels, so every global access is a contiguous row segment ----------
-        const int cw = warp - 4;
-        constexpr int nv = NC >> 2;                                // float4 per row (this CTA's channels)
-        for (int e = lane; e < (BM / NUM_CONSUMER_WARPS) * nv; e += 32) {
-            const int rr = cw + NUM_CONSUMER_WARPS * (e / nv);
-            const int lcol = (e % nv) * 4;
-            const int col = n0 + lcol;
-            const int orow = row_s[rr];
-            if (orow < 0) continue;
-            const long long ro = (long long)orow * p.cout;
-            const float4 a4 = *reinterpret_cast<const float4*>(stage_c + (size_t)rr * pitch + lcol);
-            float y[4] = {a4.x, a4.y, a4.z, a4.w};
-            if (io.pre_add) {
-                const float4 t4 = __ldg(reinterpret_cast<const float4*>(io.pre_add + ro + col));
-                y[0] += t4.x; y[1] += t4.y; y[2] += t4.z; y[3] += t4.w;
-            }
-            if (p.scale) {
-                const float4 s4 = __ldg(reinterpret_cast<const float4*>(p.scale + col));
-                const float4 h4 = __ldg(reinterpret_cast<const float4*>(p.shift + col));
-                y[0] = fmaf(y[0], s4.x, h4.x); y[1] = fmaf(y[1], s4.y, h4.y); y[2] = fmaf(y[2], s4.z, h4.z); y[3] = fmaf(y[3], s4.w, h4.w);
-            }
-            if (io.residual || io.residual_h) {
-                const float4 t4 = load_residual4(io.residual, io.residual_h, orow, p.cout, col);
-                y[0] += t4.x; y[1] += t4.y; y[2] += t4.z; y[3] += t4.w;
-            }
-            if (p.relu) {
+            for (int i = 0; i < NC / 2; ++i) tot[i] = -0.f;
+            // one flat loop over the tile's stages (offset-major, chunk-minor), the stage sequence the producers publish
+            const int n_it = n_off * p.nchunks;
+            int c = 0, in_group = 0, off_idx = 0, prev_s = -1;
+            for (int i = 0; i < n_it; ++i, ++it) {
+                const int s = it % S;
+                const uint32_t par = (it / S) & 1;
+                mbar_wait(full_b(s), par);
+                mbar_wait(full_a(s), par);
+                const uint32_t a_hi = base + (uint32_t)s * stage_bytes + (uint32_t)wg * (A_TILE / 2), a_lo = a_hi + A_TILE;
+                const uint32_t b_hi = base + (uint32_t)s * stage_bytes + 2u * A_TILE, b_lo = b_hi + b_tile;
+                const int ksteps = min(KC, ctot - c * KC) >> 4;
+                reg_fence(acc);
+                wg_stage_mma<NC>(acc, a_hi, a_lo, b_hi, b_lo, ksteps, in_group == 0 && c == 0);   // first MMA of a group overwrites
+                reg_fence(acc);
+                wgmma_wait<1>();                                      // the MMAs of the previous stage are done: release it
+                if (prev_s >= 0 && lane == 0) mbar_arrive(empty(prev_s));
+                prev_s = s;
+                if (++c < p.nchunks) continue;
+                c = 0;
+                ++off_idx;
+                if (++in_group == p.group || off_idx == n_off) {      // partial sum of this group complete -> running total
+                    wgmma_wait<0>();
+                    reg_fence(acc);
+                    if (lane == 0) mbar_arrive(empty(prev_s));
+                    prev_s = -1;
 #pragma unroll
-                for (int j = 0; j < 4; ++j) y[j] = fmaxf(y[j], 0.f);
-            }
-            if (io.out) *reinterpret_cast<float4*>(io.out + ro + col) = make_float4(y[0], y[1], y[2], y[3]);
-            if (io.out_h) store_split4(io.out_h, orow, p.cout, col, y);
-            if (io.out_gated || io.out_gated_h) {
-                if (io.gate_table) {
-                    const long long g = io.gate_idx ? __ldg(io.gate_idx + orow) : 0;
-                    const float4 g4 = __ldg(reinterpret_cast<const float4*>(io.gate_table + g * p.cout + col));
-                    y[0] *= g4.x; y[1] *= g4.y; y[2] *= g4.z; y[3] *= g4.w;
+                    for (int i = 0; i < NC / 2; ++i) tot[i] = __fadd_rn(tot[i], acc[i]);
+                    in_group = 0;
                 }
-                if (io.out_gated) *reinterpret_cast<float4*>(io.out_gated + ro + col) = make_float4(y[0], y[1], y[2], y[3]);
-                if (io.out_gated_h) store_split4(io.out_gated_h, orow, p.cout, col, y);
+            }
+            // the last stage always ends a group, so nothing is in flight here; ptxas cannot see that, and without this wait it injects one
+            // on the loop's exit edge (C7517) before the epilogue reuses the accumulator registers
+            wgmma_wait<0>();
+            // ---- totals -> the epilogue slot, [BM][NC] fp32 with the 16-byte column chunks XOR-swizzled by row (no bank conflicts on
+            //      the fragment writes nor the row reads; NC = 128 fills a stage exactly) ----------
+            const int se = it % S;
+            mbar_wait(full_b(se), (it / S) & 1);
+            mbar_wait(full_a(se), (it / S) & 1);
+            ++it;
+            float* stage_c = reinterpret_cast<float*>(gen + (size_t)se * stage_bytes);
+            {
+                const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+                for (int i = 0; i < NC / 2; i += 2) {
+                    const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3);
+                    *reinterpret_cast<float2*>(stage_c + row * NC + (((col >> 2) ^ (row & 7)) << 2) + (col & 3)) =
+                        make_float2(tot[i] * out_scale, tot[i + 1] * out_scale);
+                }
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            // ---- epilogue, coalesced: consumer warp cw owns tile rows cw, cw + 8, ... and walks their (row, 4-channel) elements with
+            //      consecutive lanes on consecutive channels, so every global access is a contiguous row segment ----------
+            const lb2_conv_io io = p.io[(x / p.nsplit) % p.npass];
+            const int n0 = (x % p.nsplit) * NC;                        // first output channel of the item
+            const int cw = warp - 4;
+            constexpr int nv = NC >> 2;                                // float4 per row (the item's channels)
+            for (int e = lane; e < (BM / NUM_CONSUMER_WARPS) * nv; e += 32) {
+                const int rr = cw + NUM_CONSUMER_WARPS * (e / nv);
+                const int lcol = (e % nv) * 4;
+                const int col = n0 + lcol;
+                const int orow = ti.row[rr];
+                if (orow < 0) continue;
+                const long long ro = (long long)orow * p.cout;
+                const float4 a4 = *reinterpret_cast<const float4*>(stage_c + rr * NC + (((lcol >> 2) ^ (rr & 7)) << 2));
+                float y[4] = {a4.x, a4.y, a4.z, a4.w};
+                if (io.pre_add) {
+                    const float4 t4 = __ldg(reinterpret_cast<const float4*>(io.pre_add + ro + col));
+                    y[0] += t4.x; y[1] += t4.y; y[2] += t4.z; y[3] += t4.w;
+                }
+                if (p.scale) {
+                    const float4 s4 = __ldg(reinterpret_cast<const float4*>(p.scale + col));
+                    const float4 h4 = __ldg(reinterpret_cast<const float4*>(p.shift + col));
+                    y[0] = fmaf(y[0], s4.x, h4.x); y[1] = fmaf(y[1], s4.y, h4.y); y[2] = fmaf(y[2], s4.z, h4.z); y[3] = fmaf(y[3], s4.w, h4.w);
+                }
+                if (io.residual || io.residual_h) {
+                    const float4 t4 = load_residual4(io.residual, io.residual_h, orow, p.cout, col);
+                    y[0] += t4.x; y[1] += t4.y; y[2] += t4.z; y[3] += t4.w;
+                }
+                if (p.relu) {
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) y[q] = fmaxf(y[q], 0.f);
+                }
+                if (io.out) *reinterpret_cast<float4*>(io.out + ro + col) = make_float4(y[0], y[1], y[2], y[3]);
+                if (io.out_h) store_split4(io.out_h, orow, p.cout, col, y);
+                if (io.out_gated || io.out_gated_h) {
+                    if (io.gate_table) {
+                        const long long g = io.gate_idx ? __ldg(io.gate_idx + orow) : 0;
+                        const float4 g4 = __ldg(reinterpret_cast<const float4*>(io.gate_table + g * p.cout + col));
+                        y[0] *= g4.x; y[1] *= g4.y; y[2] *= g4.z; y[3] *= g4.w;
+                    }
+                    if (io.out_gated) *reinterpret_cast<float4*>(io.out_gated + ro + col) = make_float4(y[0], y[1], y[2], y[3]);
+                    if (io.out_gated_h) store_split4(io.out_gated_h, orow, p.cout, col, y);
+                }
+            }
+            // the slot's next bulk copy is an async-proxy write after these generic accesses
+            fence_proxy_async();
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(empty(se));
+                mbar_arrive(info_empty(j & 1));
             }
         }
     }
@@ -338,7 +401,7 @@ static bool shape_ok(int c1, int c2, int cout, int kvol) {
 }
 
 static size_t smem_bytes(int nc, int stages) {
-    return 1024 + (size_t)stages * (2 * A_TILE + 2 * (size_t)nc * 128) + MAX_KVOL * BM * sizeof(int) + 3 * MAX_STAGES * 8 + 16 + BM * sizeof(int);
+    return 1024 + (size_t)stages * (2 * A_TILE + 2 * (size_t)nc * 128) + 2 * sizeof(TileInfo) + NUM_BARS * sizeof(uint64_t);
 }
 
 template <int NC>
@@ -346,7 +409,9 @@ static int launch(Lb2Handle* h, cudaStream_t s, const Params& p, int stages) {
     const size_t smem = smem_bytes(NC, stages);
     cudaError_t e = lb2_configure_smem(h, LB2_K_TC + (NC / 32 - 1), k_spconv_tc<NC>, (int)(227 * 1024));
     if (e != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "k_spconv_tc smem attribute: %s", cudaGetErrorString(e));
-    k_spconv_tc<NC><<<cdiv(p.mout_cap, BM) * p.npass * p.nsplit, THREADS, smem, s>>>(p);
+    // persistent: one CTA per SM, or one per work item when there are fewer
+    const unsigned grid = (unsigned)std::min<long long>(h->num_sms, (long long)cdiv(p.mout_cap, BM) * p.npass * p.nsplit);
+    k_spconv_tc<NC><<<grid, THREADS, smem, s>>>(p);
     LB2_POST_LAUNCH(h, "k_spconv_tc");
     return LB2_OK;
 }
