@@ -316,6 +316,24 @@ size_t lb2_pc_nn_scratch_bytes(int32_t nq_cap);
 int lb2_pc_tree_build(void* h, void* stream, const double* pts, int32_t n, void* tree);
 int lb2_pc_nn(void* h, void* stream, const double* q, int32_t nq, const void* tree, double* dist, int32_t* idx, void* scratch);
 
+/* Point normals as open3d 0.17's PointCloud.estimate_normals() computes them (KDTreeSearchParamKNN(30), fast_normal_computation;
+ * tools/diff_completion_pipeline.py:204-212), in two steps over a tree from lb2_pc_tree_build(pts, n):
+ *   lb2_pc_knn      exact self-k-nearest neighbours, 1 <= k <= 32 (larger k: LB2_ERR_UNSUP).  With k_eff = min(k, n), row j of
+ *                   idx (int32[n][k_eff]) lists the k_eff points nearest to point j, itself included, ordered by
+ *                   (d², index) with d² = (dx*dx + dy*dy) + dz*dz in fp64 (no FMA contraction, as lb2_pc_nn); ties go to the
+ *                   lower index.  d2 (double[n][k_eff]) receives the distances if not NULL.  n must be the tree's point count;
+ *                   if it is not, every row is written empty.  An empty slot holds index -1 and d² = +inf: the slots of a point
+ *                   with a NaN or infinite coordinate, and those past the number of finite points (the neighbours are exact for
+ *                   finite coordinates whose squared distances do not overflow; non-finite ones never fault).
+ *   lb2_pc_normals  normals[i] (double[n][3]) = FastEigen3x3 of the one-pass cumulant covariance of the k neighbours idx[i][0..k)
+ *                   (idx: int32[n][k], k = the k_eff of lb2_pc_knn): sums of x, y, z, xx, xy, xz, yy, yz, zz in neighbour order,
+ *                   divided by k, C = E[pp^T] - E[p]E[p]^T (the identity when k < 3); the eigenvector of the smallest eigenvalue,
+ *                   unoriented, (0, 0, 1) where the solver gives the zero vector, NaN where the row holds an index outside
+ *                   [0, n) (an empty lb2_pc_knn slot; nothing is read for it).  Every operation is rounded on its own, so C is
+ *                   bit-exact against a sequential host evaluation and the normal differs from one only through acos / cos. */
+int lb2_pc_knn(void* h, void* stream, const void* tree, int32_t n, int32_t k, int32_t* idx, double* d2);
+int lb2_pc_normals(void* h, void* stream, const double* pts, int32_t n, const int32_t* idx, int32_t k, double* normals);
+
 /* np.histogramdd(pts, bins, range=[-50, 50]^3) binning (metrics.py:93-101, histogram_metrics.py:11): per axis
  * bin = searchsorted(edges, x, 'right') - 1 with edges (bins + 1 fp64, np.linspace of the range) from the caller, a value equal
  * to the last edge in the last bin, points outside the range on any axis dropped.  Outputs (each optional, cleared first):

@@ -68,6 +68,7 @@ EXPORTS = [
     "lb2_pc_tree_bytes", "lb2_pc_nn_scratch_bytes", "lb2_pc_tree_build", "lb2_pc_nn", "lb2_voxel_occupancy", "lb2_occupancy_confusion",
     "lb2_occupancy_bev", "lb2_jsd_scratch_bytes", "lb2_jsd", "lb2_dist_stats_scratch_bytes", "lb2_dist_stats",
     "lb2_map_rehash", "lb2_map_scan_scratch_bytes", "lb2_map_scan",
+    "lb2_pc_knn", "lb2_pc_normals",
 ]
 
 
@@ -145,6 +146,8 @@ class Lib:
             getattr(d, f).restype = C.c_size_t
         d.lb2_pc_tree_build.argtypes = [vp, vp, vp, i32, vp]
         d.lb2_pc_nn.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp]
+        d.lb2_pc_knn.argtypes = [vp, vp, vp, i32, i32, vp, vp]
+        d.lb2_pc_normals.argtypes = [vp, vp, vp, i32, vp, i32, vp]
         d.lb2_voxel_occupancy.argtypes = [vp, vp, vp, i32, vp, i32, vp, vp, vp]
         d.lb2_occupancy_confusion.argtypes = [vp, vp, vp, vp, i64, vp]
         d.lb2_occupancy_bev.argtypes = [vp, vp, vp, i32, vp]
@@ -343,6 +346,16 @@ class Handle:
         scratch = self._bytes(self.dll.lb2_pc_nn_scratch_bytes(nq))
         self._check(self.dll.lb2_pc_nn(self.hp, self._stream(), _ptr(q), int(nq), _ptr(tree), _ptr(dist), _ptr(idx), _ptr(scratch)),
                     "lb2_pc_nn")
+
+    def pc_knn(self, tree, n, k, idx, d2=None):
+        """idx (n, min(k, n)) int32 = the nearest points of each of the tree's n points, itself included, in (d², index) order;
+        d2 the same shape fp64 (optional); 1 <= k <= 32"""
+        self._check(self.dll.lb2_pc_knn(self.hp, self._stream(), _ptr(tree), int(n), int(k), _ptr(idx), _ptr(d2)), "lb2_pc_knn")
+
+    def pc_normals(self, pts, idx, normals):
+        """normals (n, 3) fp64 = open3d FastEigen3x3 normal of the cumulant covariance of each row of `idx` (n, k) int32"""
+        n, k = idx.shape
+        self._check(self.dll.lb2_pc_normals(self.hp, self._stream(), _ptr(pts), int(n), _ptr(idx), int(k), _ptr(normals)), "lb2_pc_normals")
 
     def voxel_occupancy(self, pts, edges, bits=None, counts=None, n_in=None):
         bins = edges.shape[0] - 1

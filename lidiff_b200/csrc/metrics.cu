@@ -234,6 +234,271 @@ extern "C" int lb2_pc_nn(void* handle, void* stream, const double* q, int32_t nq
 }
 
 // ---------------------------------------------------------------------------------------------------
+// exact self-k-NN (k <= 32) over a built tree: one warp per point of the cloud, the points taken in the tree's sorted (Morton) order
+// so that consecutive warps walk the same subtrees.  Lane j holds the j-th best (d², index) so far, lexicographically ordered; a
+// leaf's 8 candidates are measured by lanes 0-7 at once and inserted one at a time by ballot + shuffle-up.  The walk is warp-uniform
+// and depth-first, nearer child first, and skips a box only when its bound is strictly greater than the k-th distance (+inf until k
+// are held), so every point tying with the k-th is seen and the (d², index) order decides.  The DFS stack also lives in the lanes:
+// lane s holds slot s (the depth of a tree over int32 points is at most 28, and the stack never holds more than depth + 1 entries).
+// The list starts from the 32 points around the query in the sorted order; a point the walk meets again is not inserted twice.
+// Non-finite coordinates never fault: a point with a NaN or infinite coordinate does not search and only finite distances enter a
+// list, so a slot nothing fills (every slot of such a point, and the slots past the number of finite points) keeps index -1, d² = +inf.
+// ---------------------------------------------------------------------------------------------------
+#define KNN_WARPS 4
+
+__device__ __forceinline__ bool knn_less(double da, int ia, double db, int ib) { return da < db || (da == db && ia < ib); }
+
+__global__ void __launch_bounds__(32 * KNN_WARPS) k_pc_knn(const unsigned long long* __restrict__ tree, int n, int k,
+                                                           int* __restrict__ out_idx, double* __restrict__ out_d2) {
+    const int t = blockIdx.x * KNN_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (t >= n) return;                                                  // whole warps only: t is warp-uniform
+    const int nleaf = reinterpret_cast<const int*>(tree + 6)[0], tree_n = reinterpret_cast<const int*>(tree + 6)[1];
+    if (tree_n != n) {                                                   // not this tree's cloud: every row is left empty
+        if (lane < k) {
+            out_idx[(size_t)t * k + lane] = -1;
+            if (out_d2) out_d2[(size_t)t * k + lane] = INFINITY;
+        }
+        return;
+    }
+    const float* nodes = reinterpret_cast<const float*>(reinterpret_cast<const char*>(tree) + PC_HDR);
+    const double4* sp = reinterpret_cast<const double4*>(nodes + (size_t)2 * nleaf * 8);
+    const double4 qp = sp[t];                                            // sorted slot t < n is a real point
+    const double qx = qp.x, qy = qp.y, qz = qp.z;
+    const int j = (int)qp.w;
+    // seed the list with the 32 points around slot t in the sorted order (Morton neighbours, mostly near): lane s measures one,
+    // a bitonic sort across the lanes orders them, and the walk starts with a k-th distance that already prunes most of the tree
+    double best = INFINITY;                                              // this lane's entry of the sorted list
+    int best_i = 0x7fffffff;
+    {
+        const int a0 = n >= 32 ? min(max(t - 16, 0), n - 32) : 0;
+        if (a0 + lane < n) {
+            const double4 sv = sp[a0 + lane];
+            const double d = pc_d2(__dsub_rn(qx, sv.x), __dsub_rn(qy, sv.y), __dsub_rn(qz, sv.z));
+            if (d < INFINITY) { best = d; best_i = (int)sv.w; }             // only finite distances enter (NaN fails too)
+        }
+#pragma unroll
+        for (int size = 2; size <= 32; size <<= 1) {
+#pragma unroll
+            for (int stride = size >> 1; stride > 0; stride >>= 1) {
+                const double od = __shfl_xor_sync(0xffffffffu, best, stride);
+                const int oi = __shfl_xor_sync(0xffffffffu, best_i, stride);
+                const bool keep_min = ((lane & stride) == 0) == ((lane & size) == 0);
+                if (keep_min ? knn_less(od, oi, best, best_i) : knn_less(best, best_i, od, oi)) { best = od; best_i = oi; }
+            }
+        }
+    }
+    double kth = __shfl_sync(0xffffffffu, best, k - 1);                  // lane k-1's distance (+inf until k are held)
+    int st_node = 0;                                                     // stack slot `lane`
+    double st_lb = 0.0;
+    int sp_n = isfinite(qx) && isfinite(qy) && isfinite(qz) ? 1 : 0;        // a non-finite point has no neighbours
+    if (lane == 0) { st_node = 1; st_lb = pc_box_d2(nodes + 8, qx, qy, qz); }
+    while (sp_n > 0) {
+        --sp_n;
+        const int node = __shfl_sync(0xffffffffu, st_node, sp_n);
+        const double lb = __shfl_sync(0xffffffffu, st_lb, sp_n);
+        if (lb == INFINITY || lb > kth) continue;
+        if (node >= nleaf) {
+            const int k0 = (node - nleaf) * PC_LEAF;
+            double d = INFINITY;
+            int pi = -1;
+            if (lane < PC_LEAF) {
+                const double2 pxy = __ldg(reinterpret_cast<const double2*>(sp + k0 + lane)),
+                              pzw = __ldg(reinterpret_cast<const double2*>(sp + k0 + lane) + 1);
+                pi = (int)pzw.y;
+                if (pi >= 0) d = pc_d2(__dsub_rn(qx, pxy.x), __dsub_rn(qy, pxy.y), __dsub_rn(qz, pzw.x));
+            }
+            const int kth_i = __shfl_sync(0xffffffffu, best_i, k - 1);
+            // only finite distances enter: a NaN or infinite point is nobody's neighbour
+            unsigned cand = __ballot_sync(0xffffffffu, pi >= 0 && d < INFINITY && knn_less(d, pi, kth, kth_i));
+            while (cand) {
+                const int c = __ffs(cand) - 1;
+                cand &= cand - 1;
+                const double dc = __shfl_sync(0xffffffffu, d, c);
+                const int ic = __shfl_sync(0xffffffffu, pi, c);
+                const double kd = __shfl_sync(0xffffffffu, best, k - 1);
+                const int ki = __shfl_sync(0xffffffffu, best_i, k - 1);
+                if (!knn_less(dc, ic, kd, ki)) continue;                 // the list moved on since the ballot
+                if (__any_sync(0xffffffffu, best_i == ic)) continue;        // already held (a seed)
+                const int pos = __popc(__ballot_sync(0xffffffffu, knn_less(best, best_i, dc, ic)));
+                const double up_d = __shfl_up_sync(0xffffffffu, best, 1);
+                const int up_i = __shfl_up_sync(0xffffffffu, best_i, 1);
+                if (lane > pos) { best = up_d; best_i = up_i; }
+                else if (lane == pos) { best = dc; best_i = ic; }
+            }
+            kth = __shfl_sync(0xffffffffu, best, k - 1);
+        } else {
+            const double l0 = pc_box_d2(nodes + (size_t)(2 * node) * 8, qx, qy, qz), l1 = pc_box_d2(nodes + (size_t)(2 * node + 1) * 8, qx, qy, qz);
+            const bool first0 = l0 <= l1;                                // nearer child popped first: pushed last
+            const int nf = first0 ? 2 * node + 1 : 2 * node, nn_ = first0 ? 2 * node : 2 * node + 1;
+            const double lf = first0 ? l1 : l0, ln = first0 ? l0 : l1;
+            if (lf != INFINITY && lf <= kth) { if (lane == sp_n) { st_node = nf; st_lb = lf; } ++sp_n; }
+            if (ln != INFINITY && ln <= kth) { if (lane == sp_n) { st_node = nn_; st_lb = ln; } ++sp_n; }
+        }
+    }
+    if (lane < k) {
+        out_idx[(size_t)j * k + lane] = best_i == 0x7fffffff ? -1 : best_i;
+        if (out_d2) out_d2[(size_t)j * k + lane] = best;
+    }
+}
+
+extern "C" int lb2_pc_knn(void* handle, void* stream, const void* tree, int32_t n, int32_t k, int32_t* idx, double* d2) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h && tree && idx && n > 0 && k >= 1, "pc_knn");
+    if (k > 32) return lb2_fail(h, LB2_ERR_UNSUP, "pc_knn: k > 32 is not supported%s", "");
+    const int ke = std::min(k, n);
+    k_pc_knn<<<cdiv(n, KNN_WARPS), 32 * KNN_WARPS, 0, (cudaStream_t)stream>>>((const unsigned long long*)tree, n, ke, idx, d2);
+    LB2_POST_LAUNCH(h, "k_pc_knn");
+    return LB2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// PCA normals as open3d 0.17 computes them (EstimateNormals with fast_normal_computation): the one-pass cumulant covariance of the
+// neighbours (ComputeCovariance) and FastEigen3x3, Geometric Tools' robust symmetric 3x3 eigensolver, for the eigenvector of the
+// smallest eigenvalue; a zero result becomes (0, 0, 1).  Every operation is an explicitly rounded fp64 intrinsic evaluated in the C++
+// source's left-to-right order (no FMA contraction), so the covariance is bit-exact and only acos / cos differ from a host libm.
+// ---------------------------------------------------------------------------------------------------
+#define RN_ADD __dadd_rn
+#define RN_SUB __dsub_rn
+#define RN_MUL __dmul_rn
+#define RN_DIV __ddiv_rn
+
+struct nv3 { double x, y, z; };
+__device__ __forceinline__ nv3 nv_cross(nv3 a, nv3 b) {
+    return {RN_SUB(RN_MUL(a.y, b.z), RN_MUL(a.z, b.y)), RN_SUB(RN_MUL(a.z, b.x), RN_MUL(a.x, b.z)), RN_SUB(RN_MUL(a.x, b.y), RN_MUL(a.y, b.x))};
+}
+__device__ __forceinline__ double nv_dot(nv3 a, nv3 b) { return RN_ADD(RN_ADD(RN_MUL(a.x, b.x), RN_MUL(a.y, b.y)), RN_MUL(a.z, b.z)); }
+__device__ __forceinline__ nv3 nv_div(nv3 a, double s) { return {RN_DIV(a.x, s), RN_DIV(a.y, s), RN_DIV(a.z, s)}; }
+
+// symmetric A = {a00, a01, a02, a11, a12, a22}
+__device__ __forceinline__ nv3 fe_evec0(const double* A, double ev) {
+    const nv3 r0 = {RN_SUB(A[0], ev), A[1], A[2]}, r1 = {A[1], RN_SUB(A[3], ev), A[4]}, r2 = {A[2], A[4], RN_SUB(A[5], ev)};
+    const nv3 c01 = nv_cross(r0, r1), c02 = nv_cross(r0, r2), c12 = nv_cross(r1, r2);
+    const double d0 = nv_dot(c01, c01), d1 = nv_dot(c02, c02), d2 = nv_dot(c12, c12);
+    double dmax = d0;
+    int imax = 0;
+    if (d1 > dmax) { dmax = d1; imax = 1; }
+    if (d2 > dmax) imax = 2;
+    if (imax == 0) return nv_div(c01, __dsqrt_rn(d0));
+    if (imax == 1) return nv_div(c02, __dsqrt_rn(d1));
+    return nv_div(c12, __dsqrt_rn(d2));
+}
+
+__device__ __forceinline__ nv3 fe_evec1(const double* A, nv3 e0, double ev1) {
+    nv3 U;
+    if (fabs(e0.x) > fabs(e0.y)) {
+        const double inv = RN_DIV(1.0, __dsqrt_rn(RN_ADD(RN_MUL(e0.x, e0.x), RN_MUL(e0.z, e0.z))));
+        U = {RN_MUL(-e0.z, inv), 0.0, RN_MUL(e0.x, inv)};
+    } else {
+        const double inv = RN_DIV(1.0, __dsqrt_rn(RN_ADD(RN_MUL(e0.y, e0.y), RN_MUL(e0.z, e0.z))));
+        U = {0.0, RN_MUL(e0.z, inv), RN_MUL(-e0.y, inv)};
+    }
+    const nv3 V = nv_cross(e0, U);
+    const nv3 r0 = {A[0], A[1], A[2]}, r1 = {A[1], A[3], A[4]}, r2 = {A[2], A[4], A[5]};
+    const nv3 AU = {nv_dot(r0, U), nv_dot(r1, U), nv_dot(r2, U)}, AV = {nv_dot(r0, V), nv_dot(r1, V), nv_dot(r2, V)};
+    double m00 = RN_SUB(nv_dot(U, AU), ev1), m01 = nv_dot(U, AV), m11 = RN_SUB(nv_dot(V, AV), ev1);
+    const double a00 = fabs(m00), a01 = fabs(m01), a11 = fabs(m11);
+    if (a00 >= a11) {
+        if (fmax(a00, a01) > 0.0) {
+            if (a00 >= a01) { m01 = RN_DIV(m01, m00); m00 = RN_DIV(1.0, __dsqrt_rn(RN_ADD(1.0, RN_MUL(m01, m01)))); m01 = RN_MUL(m01, m00); }
+            else { m00 = RN_DIV(m00, m01); m01 = RN_DIV(1.0, __dsqrt_rn(RN_ADD(1.0, RN_MUL(m00, m00)))); m00 = RN_MUL(m00, m01); }
+            return {RN_SUB(RN_MUL(m01, U.x), RN_MUL(m00, V.x)), RN_SUB(RN_MUL(m01, U.y), RN_MUL(m00, V.y)), RN_SUB(RN_MUL(m01, U.z), RN_MUL(m00, V.z))};
+        }
+        return U;
+    }
+    if (fmax(a11, a01) > 0.0) {
+        if (a11 >= a01) { m01 = RN_DIV(m01, m11); m11 = RN_DIV(1.0, __dsqrt_rn(RN_ADD(1.0, RN_MUL(m01, m01)))); m01 = RN_MUL(m01, m11); }
+        else { m11 = RN_DIV(m11, m01); m01 = RN_DIV(1.0, __dsqrt_rn(RN_ADD(1.0, RN_MUL(m11, m11)))); m11 = RN_MUL(m11, m01); }
+        return {RN_SUB(RN_MUL(m11, U.x), RN_MUL(m01, V.x)), RN_SUB(RN_MUL(m11, U.y), RN_MUL(m01, V.y)), RN_SUB(RN_MUL(m11, U.z), RN_MUL(m01, V.z))};
+    }
+    return U;
+}
+
+// FastEigen3x3 of the covariance C = {c00, c01, c02, c11, c12, c22}: eigenvector of the smallest eigenvalue, or 0 when max C == 0
+__device__ __forceinline__ nv3 fast_eigen3x3(const double* C) {
+    double mc = C[0];
+#pragma unroll
+    for (int i = 1; i < 6; ++i) mc = C[i] > mc ? C[i] : mc;
+    if (mc == 0.0) return {0.0, 0.0, 0.0};
+    double A[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) A[i] = RN_DIV(C[i], mc);
+    const double norm = RN_ADD(RN_ADD(RN_MUL(A[1], A[1]), RN_MUL(A[2], A[2])), RN_MUL(A[4], A[4]));
+    if (!(norm > 0.0)) {
+        const double s00 = RN_MUL(A[0], mc), s11 = RN_MUL(A[3], mc), s22 = RN_MUL(A[5], mc);
+        if (s00 < s11 && s00 < s22) return {1.0, 0.0, 0.0};
+        if (s11 < s00 && s11 < s22) return {0.0, 1.0, 0.0};
+        return {0.0, 0.0, 1.0};
+    }
+    const double q = RN_DIV(RN_ADD(RN_ADD(A[0], A[3]), A[5]), 3.0);
+    const double b00 = RN_SUB(A[0], q), b11 = RN_SUB(A[3], q), b22 = RN_SUB(A[5], q);
+    const double p = __dsqrt_rn(RN_DIV(RN_ADD(RN_ADD(RN_ADD(RN_MUL(b00, b00), RN_MUL(b11, b11)), RN_MUL(b22, b22)), RN_MUL(norm, 2.0)), 6.0));
+    const double c00 = RN_SUB(RN_MUL(b11, b22), RN_MUL(A[4], A[4]));
+    const double c01 = RN_SUB(RN_MUL(A[1], b22), RN_MUL(A[4], A[2]));
+    const double c02 = RN_SUB(RN_MUL(A[1], A[4]), RN_MUL(b11, A[2]));
+    const double det = RN_DIV(RN_ADD(RN_SUB(RN_MUL(b00, c00), RN_MUL(A[1], c01)), RN_MUL(A[2], c02)), RN_MUL(RN_MUL(p, p), p));
+    double half_det = RN_MUL(det, 0.5);
+    half_det = half_det < -1.0 ? -1.0 : half_det;                         // std::min(std::max(x, -1), 1)
+    half_det = 1.0 < half_det ? 1.0 : half_det;
+    const double angle = RN_DIV(acos(half_det), 3.0);
+    const double beta2 = RN_MUL(cos(angle), 2.0);
+    const double beta0 = RN_MUL(cos(RN_ADD(angle, 2.09439510239319549)), 2.0);
+    const double beta1 = -RN_ADD(beta0, beta2);
+    const double ev0 = RN_ADD(q, RN_MUL(p, beta0)), ev1 = RN_ADD(q, RN_MUL(p, beta1)), ev2 = RN_ADD(q, RN_MUL(p, beta2));
+    if (half_det >= 0.0) {
+        const nv3 e2 = fe_evec0(A, ev2);
+        if (ev2 < ev0 && ev2 < ev1) return e2;
+        const nv3 e1 = fe_evec1(A, e2, ev1);
+        if (ev1 < ev0 && ev1 < ev2) return e1;
+        return nv_cross(e1, e2);
+    }
+    const nv3 e0 = fe_evec0(A, ev0);
+    if (ev0 < ev1 && ev0 < ev2) return e0;
+    const nv3 e1 = fe_evec1(A, e0, ev1);
+    if (ev1 < ev0 && ev1 < ev2) return e1;
+    return nv_cross(e0, e1);
+}
+
+__global__ void __launch_bounds__(128) k_pc_normals(const double* __restrict__ pts, int n, const int* __restrict__ idx, int k,
+                                                    double* __restrict__ normals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int* row = idx + (size_t)i * k;
+    bool complete = true;                                                // every index of the row is a point of the cloud
+    for (int u = 0; u < k; ++u) { const int m = __ldg(row + u); complete &= m >= 0 && m < n; }
+    if (!complete) {
+        normals[3 * (size_t)i] = normals[3 * (size_t)i + 1] = normals[3 * (size_t)i + 2] = CUDART_NAN;
+        return;
+    }
+    double C[6] = {1.0, 0.0, 0.0, 1.0, 0.0, 1.0};                       // identity below 3 neighbours
+    if (k >= 3) {
+        double s[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int u = 0; u < k; ++u) {
+            const int m = __ldg(row + u);
+            const double x = __ldg(pts + 3 * (size_t)m), y = __ldg(pts + 3 * (size_t)m + 1), z = __ldg(pts + 3 * (size_t)m + 2);
+            s[0] = RN_ADD(s[0], x); s[1] = RN_ADD(s[1], y); s[2] = RN_ADD(s[2], z);
+            s[3] = RN_ADD(s[3], RN_MUL(x, x)); s[4] = RN_ADD(s[4], RN_MUL(x, y)); s[5] = RN_ADD(s[5], RN_MUL(x, z));
+            s[6] = RN_ADD(s[6], RN_MUL(y, y)); s[7] = RN_ADD(s[7], RN_MUL(y, z)); s[8] = RN_ADD(s[8], RN_MUL(z, z));
+        }
+        const double cnt = (double)k;
+#pragma unroll
+        for (int a = 0; a < 9; ++a) s[a] = RN_DIV(s[a], cnt);
+        C[0] = RN_SUB(s[3], RN_MUL(s[0], s[0])); C[3] = RN_SUB(s[6], RN_MUL(s[1], s[1])); C[5] = RN_SUB(s[8], RN_MUL(s[2], s[2]));
+        C[1] = RN_SUB(s[4], RN_MUL(s[0], s[1])); C[2] = RN_SUB(s[5], RN_MUL(s[0], s[2])); C[4] = RN_SUB(s[7], RN_MUL(s[1], s[2]));
+    }
+    nv3 v = fast_eigen3x3(C);
+    if (v.x == 0.0 && v.y == 0.0 && v.z == 0.0) v = {0.0, 0.0, 1.0};
+    normals[3 * (size_t)i] = v.x; normals[3 * (size_t)i + 1] = v.y; normals[3 * (size_t)i + 2] = v.z;
+}
+
+extern "C" int lb2_pc_normals(void* handle, void* stream, const double* pts, int32_t n, const int32_t* idx, int32_t k, double* normals) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h && pts && normals && n > 0 && k >= 0 && (idx || k == 0), "pc_normals");
+    k_pc_normals<<<cdiv(n, 128), 128, 0, (cudaStream_t)stream>>>(pts, n, idx, k, normals);
+    LB2_POST_LAUNCH(h, "k_pc_normals");
+    return LB2_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // voxel occupancy / counts with np.histogramdd's binning: bin = searchsorted(edges, x, 'right') - 1 per axis, the last edge belongs
 // to the last bin, anything outside [edges[0], edges[bins]] (or NaN) is dropped.  The arithmetic guess is corrected against the fp64
 // edge table, so membership is decided by the same comparisons numpy makes.

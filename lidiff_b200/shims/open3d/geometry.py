@@ -159,11 +159,19 @@ class PointCloud(Geometry):
         return np.asarray(self._points).max(0)
 
     def estimate_normals(self, search_param=None, fast_normal_computation=True):
-        """PCA normal of the k nearest neighbours (k = 30 as open3d's default KNN search), sign left unoriented.  Post-processing
-        only, not on the timed path; exact bucketed k-NN search (`_knn`)."""
+        """PCA normal of the k nearest neighbours (k = `knn`, else `max_nn`, else 30 as open3d's default KNN search; the radius of
+        KDTreeSearchParamHybrid is ignored), sign left unoriented.  On a GPU: open3d's cumulant covariance and FastEigen3x3 over an
+        exact (d², index)-ordered k-NN (lidiff_b200.normals.estimate_normals); that kernel takes k <= 32, so a larger knn / max_nn
+        raises ValueError there rather than running another implementation.  Without a GPU: an exact bucketed k-NN search (`_knn`)
+        and the eigenvector of torch's eigh, any k."""
         import torch
         k = getattr(search_param, "knn", None) or getattr(search_param, "max_nn", None) or 30
-        dev = "cuda" if torch.cuda.is_available() else "cpu"
+        if torch.cuda.is_available():
+            from lidiff_b200.normals import estimate_normals
+            pts = np.asarray(self._points)
+            self._normals = Vector3dVector(estimate_normals(pts, knn=k).cpu().numpy() if len(pts) else np.zeros((0, 3)))
+            return True
+        dev = "cpu"
         p = torch.as_tensor(np.asarray(self._points), dtype=torch.float32, device=dev)
         n = p.shape[0]
         k = min(k, n)

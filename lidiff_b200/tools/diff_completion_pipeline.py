@@ -1,7 +1,8 @@
 """Command-line scene completion — counterpart of the reference's
 `python3 tools/diff_completion_pipeline.py -d diff_net.ckpt -r refine_net.ckpt -T 50 -s 6.0`
 (/root/reference/lidiff/tools/diff_completion_pipeline.py:179-212): same options, same outputs
-(`results/<exp>/{diff,refine}/<scan>.ply`), plus sharding of the scans over the ranks of a torchrun job
+(`results/<exp>/{diff,refine}/<scan>.ply`; with `--normals` each PLY also carries the reference's open3d estimate_normals()
+normals as `nx ny nz`, computed on the GPU by lidiff_b200.normals), plus sharding of the scans over the ranks of a torchrun job
 (one process per GPU, scan b on rank b mod R; SURVEY.md 8e).
 
     torchrun --nproc-per-node 8 -m lidiff_b200.tools.diff_completion_pipeline -d diff.ckpt -r refine.ckpt --path ./Datasets/test
@@ -16,6 +17,7 @@ import click
 import numpy as np
 import torch
 
+from ..normals import estimate_normals
 from ..pipeline import DiffCompletion
 from ..sharding import scans_of_rank
 from ..synth import read_ply_xyz
@@ -29,11 +31,19 @@ def load_pcd(pcd_file: str) -> np.ndarray:
     raise click.ClickException(f"Point cloud format '.{pcd_file.split('.')[-1]}' not supported. (supported formats: .bin (kitti format), .ply)")
 
 
-def write_ply(path: str, pts: np.ndarray):
+def write_ply(path: str, pts: np.ndarray, normals: np.ndarray | None = None):
+    """binary little-endian PLY of fp64 `x y z` vertices, or `x y z nx ny nz` with `normals` (the layout open3d writes)"""
     pts = np.ascontiguousarray(pts, dtype=np.float64)
+    props = "property double x\nproperty double y\nproperty double z\n"
+    if normals is not None:
+        normals = np.asarray(normals, dtype=np.float64)
+        if normals.shape != pts.shape:
+            raise ValueError(f"write_ply: normals of shape {normals.shape} for points of shape {pts.shape}")
+        pts = np.concatenate([pts, normals], 1)
+        props += "property double nx\nproperty double ny\nproperty double nz\n"
     with open(path, "wb") as f:
         f.write(("ply\nformat binary_little_endian 1.0\ncomment Created by lidiff_b200\n"
-                 f"element vertex {pts.shape[0]}\nproperty double x\nproperty double y\nproperty double z\nend_header\n").encode("ascii"))
+                 f"element vertex {pts.shape[0]}\n{props}end_header\n").encode("ascii"))
         f.write(pts.astype("<f8").tobytes())
 
 
@@ -45,7 +55,8 @@ def write_ply(path: str, pts: np.ndarray):
 @click.option("--path", type=str, default="./Datasets/test/", help="directory with .ply / .bin scans")
 @click.option("--out", type=str, default="./results", help="output root")
 @click.option("--random-weights", is_flag=True, help="seeded random parameters instead of checkpoints (plumbing / benchmarking)")
-def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights):
+@click.option("--normals", is_flag=True, help="write open3d's estimate_normals() (30 nearest neighbours) as nx ny nz, as the reference does")
+def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, normals):
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
     device = torch.device("cuda", local_rank)
@@ -71,8 +82,9 @@ def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights):
         torch.cuda.synchronize()
         print(f"[rank {rank}] {name}: took {time.time() - start:.3f}s")
         stem = name.split(".")[0]
-        write_ply(f"{out}/{exp_dir}/refine/{stem}.ply", refine_scan)
-        write_ply(f"{out}/{exp_dir}/diff/{stem}.ply", diff_scan)
+        for kind, cloud in (("refine", refine_scan), ("diff", diff_scan)):
+            nrm = estimate_normals(cloud, device=device).cpu().numpy() if normals else None
+            write_ply(f"{out}/{exp_dir}/{kind}/{stem}.ply", cloud, nrm)
     if world > 1:
         import torch.distributed as dist
         dist.barrier()
