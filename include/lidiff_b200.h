@@ -138,9 +138,13 @@ typedef struct {
     float*         out_gated;   /* (m, cout) or NULL */
     const float*   pre_add;     /* (m, cout) or NULL: added to the raw convolution sum before the affine
                                    (the off-centre part computed by lb2_spconv_scatter) */
-    /* optional fp16 "split" companions (row = [C halfs hi | C halfs lo], x ~= hi + lo; same 4C bytes as fp32):
+    /* optional fp16 "split" companions (row = [C halfs hi | C halfs lo]; same 4C bytes as fp32):
        inputs let the tensor-core kernels gather with cp.async instead of converting in registers,
-       outputs are written by the epilogue next to the fp32 tensors. */
+       outputs are written by the epilogue next to the fp32 tensors.  Every producer (these epilogues, lb2_gate_mul, the
+       tensor-core kernels' own split of fp32 rows) writes the same split, RN = round to nearest-even, RN_sat = RN with
+       results clamped to +-65504:  hi = RN_sat(x), lo = RN(x - hi).  For |x| < 131024, |x - hi - lo| <= 2^-22 |x| + 2^-25 (an
+       absolute floor below |x| = 2^-3, where lo is subnormal); for larger |x| and +-inf, lo = +-inf, and NaN gives hi = lo = NaN,
+       so every output that reads a non-finite (or unrepresentable) activation is non-finite, as with LB2_ALGO_FFMA. */
     const void*    in1_h;       /* (rows_in, 2*c1) fp16 or NULL */
     const void*    in2_h;       /* (rows_in, 2*c2) fp16 or NULL */
     void*          out_h;       /* (m, 2*cout) fp16 or NULL */
@@ -210,7 +214,10 @@ int lb2_spconv_scatter_supported(int32_t c1, int32_t c2, int32_t cout, int32_t k
 int lb2_spconv_scatter(void* h, void* stream, const lb2_scatter_desc* d);
 
 /* FP16 hi/lo split (power-of-two pre-scaled) + wgmma shared-memory image of a (kvol, cin, cout) fp32 weight
- * for LB2_ALGO_TC. */
+ * for LB2_ALGO_TC: a 256-byte header ([0] max|W| as float bits, [1] the float 2^-k), then per (k, 64-channel chunk)
+ * [hi tile | lo tile], each cout rows x 128 B in the K-major SWIZZLE_128B layout, channels >= cin zero.  Values are
+ * W 2^k split as hi = RN(W 2^k), lo = RN(W 2^k - hi), with k chosen so that max|W| 2^k lies in [8192, 16384), capped at
+ * k = 126 (max|W| < 2^-113), k = 0 for all-zero W: any finite W gives a finite image and a finite, nonzero, normal header[1]. */
 size_t lb2_packed_weight_bytes(int32_t kvol, int32_t cin, int32_t cout);
 int lb2_pack_weights(void* h, void* stream, const float* weight, int32_t kvol, int32_t cin, int32_t cout,
                      void* packed);

@@ -4,7 +4,8 @@
 //     x = x_hi + x_lo (fp16 each),  w*2^k = w_hi + w_lo,   x.w ~= (x_hi.w_hi + x_lo.w_hi + x_hi.w_lo) * 2^-k
 // (22 mantissa bits per operand; the dropped x_lo.w_lo term is ~2^-22 relative.  BF16x3 costs the same
 // three MMAs and is far less accurate.  Weights are pre-scaled by a power of two per layer so their low
-// parts stay in fp16's normal range; activations saturate at +-65504.)
+// parts stay in fp16's normal range.  Activations follow tc::split2: below |x| = 2^-3 the split has an
+// absolute error floor of 2^-25; +-inf, NaN and any |x| >= 131024 make the products that read them non-finite.)
 //
 // A work item is 128 output rows x NC output channels of one guidance pass (NC = Cout, or Cout / 2 for Cout > 128).
 // Items are numbered (tile slot, pass, channel half), the half fastest; slot i is tile tile_order[i] (most expensive
@@ -366,7 +367,9 @@ __device__ __forceinline__ float weight_scale(unsigned max_bits) {
     if (!(m > 0.f) || !isfinite(m)) return 1.f;
     int e;
     frexpf(m, &e);                         // m = f * 2^e, f in [0.5, 1)
-    return ldexpf(1.f, 14 - e);            // m * scale in [8192, 16384)
+    // m * scale in [8192, 16384); below m = 2^-113 it stops at 2^126, so that the scale and header[1] = 2^-126 stay finite, nonzero
+    // and normal (nothing depends on how the build treats fp32 subnormals)
+    return ldexpf(1.f, min(14 - e, 126));
 }
 
 __global__ void k_pack_weights(const float* __restrict__ w, int kvol, int cin, int cout, int nchunks, unsigned char* __restrict__ out) {

@@ -150,18 +150,36 @@ __device__ __forceinline__ uint32_t sw128(int row, int chunk) {
     return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4));
 }
 
-// two fp32 -> packed (hi, hi) and (lo, lo) fp16 pairs.  F2FP.SATFINITE rounds each half independently to nearest-even and clamps to
-// +-65504 instead of producing inf, so inside the fp16 range the results equal the scalar split1 below bit for bit (beyond it hi
-// saturates and lo carries what it can of the rest)
-__device__ __forceinline__ uint32_t cvt_f16x2_sat(float lo_half, float hi_half) {
+// RN_sat: fp32 -> fp16 rounded to nearest-even, results beyond the fp16 range (infinities included) clamped to +-65504, NaN kept NaN
+// (cvt .satfinite); RN: the same rounding without the clamp (beyond 65504 -> +-inf).  Two values at once, x in the low half.
+__device__ __forceinline__ uint32_t cvt_f16x2_sat(float x, float y) {
     uint32_t d;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi_half), "f"(lo_half));
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(y), "f"(x));
     return d;
 }
+__device__ __forceinline__ uint32_t cvt_f16x2_rn(float x, float y) {
+    uint32_t d;
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(y), "f"(x));
+    return d;
+}
+// THE fp32 -> fp16 (hi, lo) split of the FP16x3 product: every split companion (conv epilogues, gate_mul) and every A-operand image
+// gathered from fp32 rows is written by it, so a result does not depend on which kernel produced its input or how it was gathered.
+//   hi = RN_sat(x),  lo = RN(x - hi).
+//   |x| < 131024: hi + lo = x to 2^-22 relative; below |x| = 2^-3 lo is an fp16 subnormal, so the error has an absolute floor of
+//   2^-25 (|x| < 2^-25 splits to zero).  Beyond 65504 hi saturates and lo carries the rest.
+//   |x| >= 131024, +-inf included: lo = +-inf, so every product that reads x is non-finite, as in the fp32 convolutions.
+//   NaN: hi = lo = NaN.
+// Two values per call: x0 in the low halves of hi and lo, x1 in the high halves.
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
     hi = cvt_f16x2_sat(x0, x1);
     const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-    lo = cvt_f16x2_sat(x0 - f.x, x1 - f.y);
+    lo = cvt_f16x2_rn(x0 - f.x, x1 - f.y);
+}
+__device__ __forceinline__ void split1(float x, __half& hi, __half& lo) {
+    uint32_t h, l;
+    split2(x, 0.f, h, l);
+    hi = __ushort_as_half((unsigned short)(h & 0xFFFFu));
+    lo = __ushort_as_half((unsigned short)(l & 0xFFFFu));
 }
 __device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& hi, uint4& lo) {
     split2(a.x, a.y, hi.x, lo.x);
@@ -170,13 +188,6 @@ __device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& 
     split2(b.z, b.w, hi.w, lo.w);
 }
 
-
-// fp32 -> (hi, lo) fp16 pair, saturating at the fp16 range
-__device__ __forceinline__ void split1(float x, __half& hi, __half& lo) {
-    x = fminf(fmaxf(x, -65504.f), 65504.f);
-    hi = __float2half_rn(x);
-    lo = __float2half_rn(x - __half2float(hi));
-}
 // write 4 consecutive channels of a split companion row: hi halfs at row[col], lo halfs at row[c + col]
 __device__ __forceinline__ void store_split4(void* base, long long row, int c, int col, const float (&y)[4]) {
     __half* rp = reinterpret_cast<__half*>(base) + row * 2 * c;

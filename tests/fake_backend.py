@@ -9,6 +9,7 @@ import numpy as np
 import torch
 
 from oracle import me_cpu as ome
+from split_numerics import split
 
 
 def _arr(ptr, shape, ctype, npdtype):
@@ -44,10 +45,7 @@ def _write_act(f_ptr, h_ptr, rows, c, y):
     if f_ptr:
         _f(f_ptr, (rows, c))[:] = y32.numpy()
     if h_ptr:
-        y32 = y32.clamp(-65504.0, 65504.0)
-        hi = y32.half()
-        lo = (y32 - hi.float()).half()
-        _h(h_ptr, (rows, 2 * c))[:] = torch.cat([hi, lo], 1).numpy()
+        _h(h_ptr, (rows, 2 * c))[:] = torch.cat(split(y32), 1).numpy()
 
 
 class FakeHandle:
@@ -320,9 +318,7 @@ class FakeHandle:
         if out is not None:
             out[:M] = y
         if out_h is not None:
-            y = y.clamp(-65504.0, 65504.0)
-            hi = y.half()
-            out_h[:M] = torch.cat([hi, (y - hi.float()).half()], 1)
+            out_h[:M] = torch.cat(split(y), 1)
 
     def head_mlp(self, x, ldx, x_pass_stride, w0, b0, w1, b1, m_cap, d_m, n_in, n_hid, n_out, out_act, npass, y, ldy, y_pass_stride):
         self.launches += 1
