@@ -42,6 +42,7 @@ constexpr int NUM_CONSUMER_WARPS = 8;
 constexpr int STEP_BUDGET = 64;       // max chained MMA steps per accumulation group
 constexpr int MAX_KVOL = 27;
 constexpr int MAX_STAGES = 4;
+constexpr int EPI_BATCH = 4;         // epilogue elements per lane whose loads are in flight together
 
 struct Params {
     int c1, c2, cout, kvol;
@@ -296,47 +297,71 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
             }
             asm volatile("bar.sync 1, 256;" ::: "memory");
             // ---- epilogue, coalesced: consumer warp cw owns tile rows cw, cw + 8, ... and walks their (row, 4-channel) elements with
-            //      consecutive lanes on consecutive channels, so every global access is a contiguous row segment ----------
+            //      consecutive lanes on consecutive channels, so every global access is a contiguous row segment.  A lane takes its
+            //      elements in batches of EPI_BATCH: every load of a batch (pre_add, BN affine, residual, gate index) is issued before
+            //      any of its arithmetic, the gate rows right after their indices, then the stores.  One element at a time, each
+            //      element waited for its loads and its gate index -> gate row chain in turn, with the tensor cores idle.  The
+            //      arithmetic of an element is unchanged.  ----------
             const lb2_conv_io io = p.io[(x / p.nsplit) % p.npass];
             const int n0 = (x % p.nsplit) * NC;                        // first output channel of the item
             const int cw = warp - 4;
             constexpr int nv = NC >> 2;                                // float4 per row (the item's channels)
-            for (int e = lane; e < (BM / NUM_CONSUMER_WARPS) * nv; e += 32) {
-                const int rr = cw + NUM_CONSUMER_WARPS * (e / nv);
-                const int lcol = (e % nv) * 4;
-                const int col = n0 + lcol;
-                const int orow = ti.row[rr];
-                if (orow < 0) continue;
-                const long long ro = (long long)orow * p.cout;
-                const float4 a4 = *reinterpret_cast<const float4*>(stage_c + rr * NC + (((lcol >> 2) ^ (rr & 7)) << 2));
-                float y[4] = {a4.x, a4.y, a4.z, a4.w};
-                if (io.pre_add) {
-                    const float4 t4 = __ldg(reinterpret_cast<const float4*>(io.pre_add + ro + col));
-                    y[0] += t4.x; y[1] += t4.y; y[2] += t4.z; y[3] += t4.w;
-                }
-                if (p.scale) {
-                    const float4 s4 = __ldg(reinterpret_cast<const float4*>(p.scale + col));
-                    const float4 h4 = __ldg(reinterpret_cast<const float4*>(p.shift + col));
-                    y[0] = fmaf(y[0], s4.x, h4.x); y[1] = fmaf(y[1], s4.y, h4.y); y[2] = fmaf(y[2], s4.z, h4.z); y[3] = fmaf(y[3], s4.w, h4.w);
-                }
-                if (io.residual || io.residual_h) {
-                    const float4 t4 = load_residual4(io.residual, io.residual_h, orow, p.cout, col);
-                    y[0] += t4.x; y[1] += t4.y; y[2] += t4.z; y[3] += t4.w;
-                }
-                if (p.relu) {
+            constexpr int PER_LANE = (BM / NUM_CONSUMER_WARPS) * nv / 32;
+            static_assert(PER_LANE % EPI_BATCH == 0, "a lane's elements come in whole batches");
+            const bool has_res = io.residual || io.residual_h;
+            const bool gated = io.out_gated || io.out_gated_h;
+            const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int e0 = 0; e0 < PER_LANE; e0 += EPI_BATCH) {
+                int orow[EPI_BATCH], col[EPI_BATCH];
+                long long gi[EPI_BATCH];
+                float4 a4[EPI_BATCH], pre4[EPI_BATCH], s4[EPI_BATCH], h4[EPI_BATCH], res4[EPI_BATCH], g4[EPI_BATCH];
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) y[q] = fmaxf(y[q], 0.f);
+                for (int b = 0; b < EPI_BATCH; ++b) {
+                    const int e = lane + 32 * (e0 + b);
+                    const int rr = cw + NUM_CONSUMER_WARPS * (e / nv);
+                    const int lcol = (e % nv) * 4;
+                    col[b] = n0 + lcol;
+                    orow[b] = ti.row[rr];
+                    const bool live = orow[b] >= 0;
+                    const long long ro = (long long)orow[b] * p.cout;
+                    a4[b] = *reinterpret_cast<const float4*>(stage_c + rr * NC + (((lcol >> 2) ^ (rr & 7)) << 2));
+                    pre4[b] = (live && io.pre_add) ? __ldg(reinterpret_cast<const float4*>(io.pre_add + ro + col[b])) : zero4;
+                    s4[b] = p.scale ? __ldg(reinterpret_cast<const float4*>(p.scale + col[b])) : zero4;
+                    h4[b] = p.scale ? __ldg(reinterpret_cast<const float4*>(p.shift + col[b])) : zero4;
+                    res4[b] = (live && has_res) ? load_residual4(io.residual, io.residual_h, orow[b], p.cout, col[b]) : zero4;
+                    gi[b] = (live && gated && io.gate_table && io.gate_idx) ? __ldg(io.gate_idx + orow[b]) : 0;
                 }
-                if (io.out) *reinterpret_cast<float4*>(io.out + ro + col) = make_float4(y[0], y[1], y[2], y[3]);
-                if (io.out_h) store_split4(io.out_h, orow, p.cout, col, y);
-                if (io.out_gated || io.out_gated_h) {
-                    if (io.gate_table) {
-                        const long long g = io.gate_idx ? __ldg(io.gate_idx + orow) : 0;
-                        const float4 g4 = __ldg(reinterpret_cast<const float4*>(io.gate_table + g * p.cout + col));
-                        y[0] *= g4.x; y[1] *= g4.y; y[2] *= g4.z; y[3] *= g4.w;
+#pragma unroll
+                for (int b = 0; b < EPI_BATCH; ++b)
+                    g4[b] = (orow[b] >= 0 && gated && io.gate_table) ? __ldg(reinterpret_cast<const float4*>(io.gate_table + gi[b] * p.cout + col[b])) : zero4;
+#pragma unroll
+                for (int b = 0; b < EPI_BATCH; ++b) {
+                    if (orow[b] < 0) continue;
+                    const long long ro = (long long)orow[b] * p.cout;
+                    float y[4] = {a4[b].x, a4[b].y, a4[b].z, a4[b].w};
+                    if (io.pre_add) {
+                        y[0] += pre4[b].x; y[1] += pre4[b].y; y[2] += pre4[b].z; y[3] += pre4[b].w;
                     }
-                    if (io.out_gated) *reinterpret_cast<float4*>(io.out_gated + ro + col) = make_float4(y[0], y[1], y[2], y[3]);
-                    if (io.out_gated_h) store_split4(io.out_gated_h, orow, p.cout, col, y);
+                    if (p.scale) {
+                        y[0] = fmaf(y[0], s4[b].x, h4[b].x); y[1] = fmaf(y[1], s4[b].y, h4[b].y);
+                        y[2] = fmaf(y[2], s4[b].z, h4[b].z); y[3] = fmaf(y[3], s4[b].w, h4[b].w);
+                    }
+                    if (has_res) {
+                        y[0] += res4[b].x; y[1] += res4[b].y; y[2] += res4[b].z; y[3] += res4[b].w;
+                    }
+                    if (p.relu) {
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) y[q] = fmaxf(y[q], 0.f);
+                    }
+                    if (io.out) *reinterpret_cast<float4*>(io.out + ro + col[b]) = make_float4(y[0], y[1], y[2], y[3]);
+                    if (io.out_h) store_split4(io.out_h, orow[b], p.cout, col[b], y);
+                    if (gated) {
+                        if (io.gate_table) {
+                            y[0] *= g4[b].x; y[1] *= g4[b].y; y[2] *= g4[b].z; y[3] *= g4[b].w;
+                        }
+                        if (io.out_gated) *reinterpret_cast<float4*>(io.out_gated + ro + col[b]) = make_float4(y[0], y[1], y[2], y[3]);
+                        if (io.out_gated_h) store_split4(io.out_gated_h, orow[b], p.cout, col[b], y);
+                    }
                 }
             }
             // the slot's next bulk copy is an async-proxy write after these generic accesses
