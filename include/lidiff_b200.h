@@ -309,6 +309,15 @@ int lb2_guidance_dpm_step(void* h, void* stream, const float* eps_c, const float
 int lb2_farthest_point_sample(void* h, void* stream, const double* pts, int32_t n, int32_t n_samples,
                               int32_t* out_idx, double* dist_scratch);
 
+/* Batched farthest point sampling: n_scans ragged scans, scan b = pts rows [d_offsets[b], d_offsets[b+1]) (d_offsets: device
+ * int64[n_scans+1]), max_n >= every scan's size, n_samples <= every scan's size.  out_idx (n_scans, n_samples) int32 holds each
+ * scan's selection order in scan-local indices, bit-identical to lb2_farthest_point_sample on that scan.  One thread-block
+ * cluster per scan with the scan's coordinates in shared memory, so the scans run concurrently; a scan may have at most
+ * lb2_fps_batched_capacity(h) points (0: the device cannot run the cluster). */
+int64_t lb2_fps_batched_capacity(void* h);
+int lb2_farthest_point_sample_batched(void* h, void* stream, const double* pts, const int64_t* d_offsets, int32_t n_scans,
+                                      int32_t max_n, int32_t n_samples, int32_t* out_idx);
+
 /* ---- evaluation metrics — lidiff/utils/metrics.py:63-221, histogram_metrics.py:7-51, eval_path.py:65-170.
  * Points are fp64 rows (n, 3).  Every result is deterministic: integer counts, fp64 sums in a fixed order. */
 

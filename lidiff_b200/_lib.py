@@ -68,7 +68,7 @@ EXPORTS = [
     "lb2_pc_tree_bytes", "lb2_pc_nn_scratch_bytes", "lb2_pc_tree_build", "lb2_pc_nn", "lb2_voxel_occupancy", "lb2_occupancy_confusion",
     "lb2_occupancy_bev", "lb2_jsd_scratch_bytes", "lb2_jsd", "lb2_dist_stats_scratch_bytes", "lb2_dist_stats",
     "lb2_map_rehash", "lb2_map_scan_scratch_bytes", "lb2_map_scan",
-    "lb2_pc_knn", "lb2_pc_normals",
+    "lb2_pc_knn", "lb2_pc_normals", "lb2_fps_batched_capacity", "lb2_farthest_point_sample_batched",
 ]
 
 
@@ -140,6 +140,9 @@ class Lib:
         d.lb2_head_mlp.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, vp, i64, i64]
         d.lb2_guidance_dpm_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, DpmCoef, vp, vp, vp, vp]
         d.lb2_farthest_point_sample.argtypes = [vp, vp, vp, i32, i32, vp, vp]
+        d.lb2_fps_batched_capacity.argtypes = [vp]
+        d.lb2_fps_batched_capacity.restype = C.c_int64
+        d.lb2_farthest_point_sample_batched.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp]
         for f, a in (("lb2_pc_tree_bytes", i32), ("lb2_pc_nn_scratch_bytes", i32), ("lb2_jsd_scratch_bytes", i64),
                      ("lb2_dist_stats_scratch_bytes", i32)):
             getattr(d, f).argtypes = [a]
@@ -328,6 +331,14 @@ class Handle:
     def farthest_point_sample(self, pts, n, n_samples, out_idx, dist):
         self._check(self.dll.lb2_farthest_point_sample(self.hp, self._stream(), _ptr(pts), int(n), int(n_samples), _ptr(out_idx), _ptr(dist)),
                     "lb2_farthest_point_sample")
+
+    def fps_batched_capacity(self) -> int:
+        """most points a scan may have in farthest_point_sample_batched (0: the device cannot run its cluster)"""
+        return int(self.dll.lb2_fps_batched_capacity(self.hp))
+
+    def farthest_point_sample_batched(self, pts, offsets, n_scans, max_n, n_samples, out_idx):
+        self._check(self.dll.lb2_farthest_point_sample_batched(self.hp, self._stream(), _ptr(pts), _ptr(offsets), int(n_scans), int(max_n),
+                                                               int(n_samples), _ptr(out_idx)), "lb2_farthest_point_sample_batched")
 
     # -- evaluation metrics (fp64 (n, 3) contiguous point tensors) ---------------------------------------------------------------
     def _bytes(self, nbytes):

@@ -8,6 +8,7 @@
 #include "common.cuh"
 #include <float.h>
 #include <algorithm>
+#include <cooperative_groups.h>
 #include "tc_common.cuh"
 
 // ---------------------------------------------------------------------------------------------------
@@ -772,5 +773,135 @@ extern "C" int lb2_farthest_point_sample(void* handle, void* stream, const doubl
     }
     k_fps<<<1, FPS_THREADS, 0, s>>>(pts, n, n_samples, out_idx, dist_scratch);
     LB2_POST_LAUNCH(h, "k_fps");
+    return LB2_OK;
+}
+
+// ---- batched: one thread-block cluster per scan, the scan on-chip -----------------------------------------------
+// CTA r of a cluster owns the points [r*slice, (r+1)*slice) of its scan: coordinates in shared memory (SoA fp64), running
+// distances in registers (FPS_CL_PPT per thread).  Each sample: thread argmax, warp and CTA reduction, the CTA's best goes
+// into its own shared slot, one barrier.cluster, and every warp reduces the cluster's slots through distributed shared
+// memory.  The slots are double-buffered by sample parity: a CTA writes slot[p] of sample it+2 only after the barrier of
+// sample it+1, which every CTA passes after it has read slot[p] of sample it.  Same arithmetic and tie rule as k_fps_coop.
+#define FPS_CL_PPT 9
+#define FPS_CL_SLICE (FPS_THREADS * FPS_CL_PPT)          // 9216 points, 216 KB of coordinates per CTA
+
+__global__ void __launch_bounds__(FPS_THREADS, 1) k_fps_cluster(const double* __restrict__ pts, const int64_t* __restrict__ offsets,
+                                                                 int slice, int n_samples, int* __restrict__ out_idx) {
+    namespace cg = cooperative_groups;
+    extern __shared__ double fc_smem[];
+    __shared__ double s_val[FPS_THREADS / 32];
+    __shared__ int s_idx[FPS_THREADS / 32];
+    __shared__ FpsBest s_slot[2];
+    cg::cluster_group cl = cg::this_cluster();
+    const int cs = (int)cl.num_blocks(), rank = (int)cl.block_rank();
+    const int scan = blockIdx.x / cs;
+    const long long off = offsets[scan];
+    const int n = (int)(offsets[scan + 1] - off);
+    const double* p = pts + 3 * off;
+    double* sx = fc_smem;
+    double* sy = sx + slice;
+    double* sz = sy + slice;
+    const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+    const int base = rank * slice, cnt = max(0, min(slice, n - base));
+    for (int j = t; j < cnt; j += FPS_THREADS) {
+        sx[j] = p[3 * (long long)(base + j)]; sy[j] = p[3 * (long long)(base + j) + 1]; sz[j] = p[3 * (long long)(base + j) + 2];
+    }
+    double dist[FPS_CL_PPT];
+#pragma unroll
+    for (int q = 0; q < FPS_CL_PPT; ++q) dist[q] = (t + q * FPS_THREADS < cnt) ? DBL_MAX : -1.0;   // -1: slot unused, can never win
+    __syncthreads();
+    int cur = 0;
+    for (int it = 0; it < n_samples; ++it) {
+        if (rank == 0 && t == 0) out_idx[(long long)scan * n_samples + it] = cur;
+        // the centre from global memory (L2): carrying it in the cluster slots instead measured 1.8x slower (DESIGN.md §3)
+        const double cx = __ldg(p + 3 * (long long)cur), cy = __ldg(p + 3 * (long long)cur + 1), cz = __ldg(p + 3 * (long long)cur + 2);
+        double bv = -1.0; int bi = 0x7fffffff;
+#pragma unroll
+        for (int q = 0; q < FPS_CL_PPT; ++q) {
+            if (dist[q] >= 0.0) {
+                const int j = t + q * FPS_THREADS;
+                const double dx = sx[j] - cx, dy = sy[j] - cy, dz = sz[j] - cz;
+                const double d = fmin(dist[q], __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
+                dist[q] = d;
+                if (d > bv) { bv = d; bi = base + j; }                 // ascending index per thread
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const double ov = __shfl_xor_sync(0xffffffffu, bv, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+        }
+        if (lane == 0) { s_val[w] = bv; s_idx[w] = bi; }
+        __syncthreads();
+        if (w == 0) {
+            bv = s_val[lane]; bi = s_idx[lane];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const double ov = __shfl_xor_sync(0xffffffffu, bv, o);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+            }
+            if (lane == 0) { s_slot[it & 1].d = bv; s_slot[it & 1].idx = bi; }
+        }
+        cl.sync();                                                     // barrier.cluster arrive.release / wait.acquire
+        bv = -1.0; bi = 0x7fffffff;
+        if (lane < cs) {
+            const FpsBest* r = cl.map_shared_rank(&s_slot[it & 1], lane);
+            bv = r->d; bi = r->idx;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const double ov = __shfl_xor_sync(0xffffffffu, bv, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+        }
+        cur = bi;
+    }
+    cl.sync();                                                         // no CTA exits while another may still read its slots
+}
+
+// cluster size for the batched kernel: 16 (non-portable) where the device can co-schedule it, else 8; 0 if neither
+static int fps_cluster_size(Lb2Handle* h) {
+    static const size_t smem = (size_t)3 * FPS_CL_SLICE * sizeof(double);
+    if (lb2_configure_smem(h, LB2_K_FPS_CLUSTER, k_fps_cluster, (int)smem) != cudaSuccess) return 0;
+    if (cudaFuncSetAttribute(k_fps_cluster, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
+    for (int cs = 16; cs >= 8; cs /= 2) {
+        cudaLaunchConfig_t cfg = {};
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.gridDim = dim3(cs); cfg.blockDim = dim3(FPS_THREADS); cfg.dynamicSmemBytes = smem; cfg.attrs = attr; cfg.numAttrs = 1;
+        int nclusters = 0;
+        if (cudaOccupancyMaxActiveClusters(&nclusters, k_fps_cluster, &cfg) == cudaSuccess && nclusters > 0) return cs;
+        (void)cudaGetLastError();
+    }
+    return 0;
+}
+
+extern "C" int64_t lb2_fps_batched_capacity(void* handle) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    if (!h) return 0;
+    return (int64_t)fps_cluster_size(h) * FPS_CL_SLICE;
+}
+
+extern "C" int lb2_farthest_point_sample_batched(void* handle, void* stream, const double* pts, const int64_t* d_offsets, int32_t n_scans,
+                                                 int32_t max_n, int32_t n_samples, int32_t* out_idx) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h && pts && d_offsets && out_idx && n_scans > 0 && max_n > 0 && n_samples > 0 && n_samples <= max_n, "fps_batched");
+    const int cs = fps_cluster_size(h);
+    if (cs == 0) return lb2_fail(h, LB2_ERR_CUDA, "fps_batched: the device cannot run an 8-CTA cluster with %s of shared memory", "216 KB");
+    LB2_REQUIRE(h, (long long)max_n <= (long long)cs * FPS_CL_SLICE, "fps_batched: a scan exceeds lb2_fps_batched_capacity()");
+    LB2_REQUIRE(h, (long long)n_scans * cs <= 0x7fffffffLL, "fps_batched: too many scans");
+    const int slice = (max_n + cs - 1) / cs;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)(n_scans * cs)); cfg.blockDim = dim3(FPS_THREADS);
+    cfg.dynamicSmemBytes = (size_t)3 * slice * sizeof(double); cfg.stream = (cudaStream_t)stream; cfg.attrs = attr; cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, k_fps_cluster, pts, d_offsets, slice, (int)n_samples, (int*)out_idx);
+    if (e != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "k_fps_cluster: %s", cudaGetErrorString(e));
+    LB2_POST_LAUNCH(h, "k_fps_cluster");
     return LB2_OK;
 }

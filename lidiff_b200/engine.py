@@ -252,10 +252,19 @@ class _PairLookup:
 class DenoiseEngine:
     def __init__(self, sd_enc: dict, sd_diff: dict, *, device="cuda", n_points=180000, denoising_steps=50,
                  cond_weight=6.0, resolution=0.05, t_steps=1000, beta_start=3.5e-5, beta_end=0.007,
-                 div_mode=1, conv_algo=_lib.ALGO_AUTO, batch_coord=0.0, sd_refine: dict | None = None, max_range=50.0):
+                 div_mode=1, conv_algo=_lib.ALGO_AUTO, batch_coord=0.0, sd_refine: dict | None = None, max_range=50.0, batch=1):
+        """batch=B: B scans of n_points points each share every launch (batch column b of the coordinate keys, capacity B*n_points
+        rows); batch=1 is the single-scan engine."""
         self.device = torch.device(device)
-        self.h = _lib.get_handle(self.device)
         self.N = int(n_points)
+        self.B = int(batch)
+        self.cap = self.B * self.N
+        if self.B != 1:
+            _check_batch(self.B, self.N, self.device)
+        self.h = _lib.get_handle(self.device)
+        # batch column of every point row (None for B = 1: column 0 is written as 0, as the single-scan engine always did)
+        self._bcol = None if self.B == 1 else \
+            torch.arange(self.B, dtype=torch.float32, device=self.device).repeat_interleave(self.N).contiguous()
         self.w = float(cond_weight)
         self.resolution = float(resolution)
         self.div_mode = int(div_mode)
@@ -292,7 +301,7 @@ class DenoiseEngine:
         self._acts = {}
         self._perm_lookup = {}
         self._tile_order_lookup = {}
-        self.geom = Geometry(h, self.N, with_up=True)
+        self.geom = Geometry(h, self.cap, with_up=True)
         self._perm_lookup = self.geom.perm_of
         self._mask_lookup = self.geom.mask_of
         self._tile_order_lookup = self.geom.tile_order_of
@@ -560,7 +569,10 @@ class DenoiseEngine:
     # ---- conditioning ------------------------------------------------------------------------------------
     def _prepare_uncond(self):
         """x_uncond = all-zero points -> one voxel at the origin with zero feature; its encoder output is
-        a single 256-vector that depends on the weights only (App. D.2).  Gate rows for all steps."""
+        a single 256-vector that depends on the weights only (App. D.2).  Gate rows for all steps.
+        A batch of B scans has B such voxels, one per batch column, each the only voxel of its batch: the kernel maps never
+        join two batches and eval BatchNorm is a per-channel affine, so every one of them has the same encoder output and the
+        gate multiplies of every batch read this one table row (gate index NULL)."""
         dev = self.device
         g1 = Geometry(self.h, 16, with_up=False, use_pairs=False)
         coords = torch.zeros((16, 4), dtype=torch.float32, device=dev)
@@ -580,9 +592,11 @@ class DenoiseEngine:
             del self._acts[k]
 
     def set_condition(self, scan: torch.Tensor):
-        """scan (N,3): the conditioning point cloud (x_cond).  Runs MinkGlobalEnc once (App. D.2)."""
-        dev, N = self.device, scan.shape[0]
-        pts = scan.to(device=dev, dtype=torch.float32).contiguous()
+        """scan (N,3): the conditioning point cloud (x_cond); (B*N,3) or (B,N,3) for a batch engine, scan b in batch column b.
+        Runs MinkGlobalEnc once (App. D.2)."""
+        dev = self.device
+        pts = scan.reshape(-1, 3).to(device=dev, dtype=torch.float32).contiguous()
+        N = pts.shape[0]
         if self.geom_cond is None or self.geom_cond.n_cap != N:
             self._graphs.clear()
             self.geom_cond = Geometry(self.h, N, with_up=False, use_pairs=False)
@@ -590,7 +604,7 @@ class DenoiseEngine:
             self._mask_lookup = ChainMap(self.geom.mask_of, self.geom_cond.mask_of)
             self._tile_order_lookup = ChainMap(self.geom.tile_order_of, self.geom_cond.tile_order_of)
         coords = self.buf("cond.coords", (N, 4))
-        coords[:, 0] = 0
+        coords[:, 0] = 0 if self._bcol is None else self._bcol
         self.h.quantize(pts, self.resolution, self.div_mode, self.buf("cond.q", (N, 3)))
         coords[:, 1:] = self._bufs["cond.q"]
         g = self.geom_cond
@@ -601,13 +615,14 @@ class DenoiseEngine:
         self.part_F = skips[4].f[0]                                    # (N cap, 256), rows valid < d_n[4]
         self.part_C, self.part_dn, self.part_grid = g.C[4], g.d_n[4], g.grid[4]
         self.part_cap = N
-        # box hierarchy over the scan's stride-16 voxels: built once per scan, into the same buffer (captured step graphs point at it)
+        # box hierarchy over the scan's stride-16 voxels (of all B scans: its nodes carry batch ranges and the search never
+        # leaves the query's batch, the reference's rule whenever a query's in-batch best d^2 is below (2 max C)^2, DESIGN.md): built once per scan, into the same buffer (captured step graphs point at it)
         self.part_tree = self.h.nn_tree(self.part_C, self.part_dn, N, out=getattr(self, "part_tree", None))
         self.A_cond = self._part_A(self.part_F, N, self.part_dn, "c")
 
     # ---- one denoising step ----------------------------------------------------------------------------------
     def step(self, i: int, x_t, x_next, coords, coords_next, x_init, noise_i, x0_state, eps_out=None):
-        h, N, g = self.h, self.N, self.geom
+        h, N, g = self.h, self.cap, self.geom
         self._conv_counter = 0
         nn = [None] * 5
         tabs_box = []
@@ -680,13 +695,14 @@ class DenoiseEngine:
         self._have_x0 = True
         cf = DpmCoef(c["c_sample"], c["c_x0"], c["c_noise"], c["sigma_s"], c["alpha_s"], c["inv_r0"] if second else 0.0,
                      self.w, self.resolution, 1 if second else 0, self.div_mode, 1)
-        h.guidance_dpm_step(eps[0], eps[1], g.inv[0], x_t, x_init, noise_i, x0_state, N, cf, eps_out, x_next, coords_next)
+        h.guidance_dpm_step(eps[0], eps[1], g.inv[0], x_t, x_init, noise_i, x0_state, N, cf, eps_out, x_next, coords_next, self._bcol)
 
     # ---- the loop (completion_loop, pipeline:155-169) -----------------------------------------------------------
     def start(self, x_init: torch.Tensor, x_feats: torch.Tensor, fresh: bool = True):
         """condition on the scan and load the noisy start; returns the loop state dict.  fresh=False keeps the multistep
-        state (last x0 prediction) of the previous trajectory like the reference's never-reset scheduler does."""
-        dev, N = self.device, self.N
+        state (last x0 prediction) of the previous trajectory like the reference's never-reset scheduler does (slot-wise in a
+        batch: scan b carries the x0 of the previous trajectory of slot b).  x_init / x_feats (B,N,3) for a batch engine."""
+        dev, N = self.device, self.cap
         if fresh:
             self._have_x0 = False
         x_src = x_init.reshape(-1, 3)
@@ -697,7 +713,7 @@ class DenoiseEngine:
         st = dict(x_init=x_init, xa=self.buf("x_a", (N, 3)), xb=self.buf("x_b", (N, 3)), ca=self.buf("c_a", (N, 4)),
                   cb=self.buf("c_b", (N, 4)), x0s=self.buf("x0_state", (N, 3), torch.float64), i=0)
         st["xa"].copy_(x_feats.reshape(-1, 3).to(device=dev, dtype=torch.float32))
-        st["ca"][:, 0] = 0
+        st["ca"][:, 0] = 0 if self._bcol is None else self._bcol
         self.h.quantize(st["xa"], self.resolution, self.div_mode, self.buf("q0", (N, 3)))
         st["ca"][:, 1:] = self._bufs["q0"]
         return st
@@ -709,7 +725,7 @@ class DenoiseEngine:
         i = st["i"] % self.T
         graphed = self.use_graphs and self.conv_events is None and self.layer_log is None and self.pair_hist is None
         if host_noise is not None or graphed:
-            nbuf = self.buf("noise_in", (self.N, 3))
+            nbuf = self.buf("noise_in", (self.cap, 3))
             nbuf.copy_(host_noise if host_noise is not None else noise_i, non_blocking=True)
             noise_i = nbuf
         if not graphed or self._eager_steps < 1:
@@ -742,16 +758,18 @@ class DenoiseEngine:
         return self.h.launch_count() - self._captured_launches + self.replayed_launches
 
     def run(self, x_init: torch.Tensor, x_feats: torch.Tensor, step_noise=None, n_steps=None, return_device=False, fresh=True):
-        """x_init (1,N,3) fp64 conditioning scan, x_feats (1,N,3) noisy start.  Returns final x_t.F (N,3)."""
+        """x_init (1,N,3) fp64 conditioning scan, x_feats (1,N,3) noisy start ((B,N,3) each for a batch engine, step_noise
+        (T,B,N,3)).  Returns final x_t.F (N,3) ((B*N,3), scan b in rows b*N..)."""
         dev, N = self.device, self.N
         st = self.start(x_init, x_feats, fresh=fresh)
         T = self.T if n_steps is None else n_steps
         if step_noise is not None:
-            step_noise = step_noise.reshape(-1, N, 3).to(device=dev, dtype=torch.float32).contiguous()
+            step_noise = step_noise.reshape(-1, self.cap, 3).to(device=dev, dtype=torch.float32).contiguous()
         for i in range(T):
             # without injected noise: one fp32 draw per step, in the order diffusers' step() draws it (the operator path and the
             # reference consume the torch RNG stream identically); no (T, N, 3) tensor is materialised (2.2 GB at T = 1000)
-            nz = step_noise[i] if step_noise is not None else torch.randn((1, N, 3), device=dev, dtype=torch.float32)[0]
+            # a batch draws (B, N, 3) once per step, as diffusers' step() does inside the reference's batched p_sample_loop
+            nz = step_noise[i] if step_noise is not None else torch.randn((self.B, N, 3), device=dev, dtype=torch.float32).reshape(-1, 3)
             self.advance(st, nz)
         if return_device:
             return st["xa"]
@@ -772,13 +790,14 @@ class DenoiseEngine:
         keep = (dist < self.max_range) & (z < max_z) & (z > min_z)
         return completed[keep].contiguous()
 
-    def refine_offsets(self, pts: torch.Tensor) -> torch.Tensor:
+    def refine_offsets(self, pts: torch.Tensor, batch_col: torch.Tensor | None = None) -> torch.Tensor:
         """refine_forward (pipeline:134-138, MinkUNet.forward minkunet.py:596-619) on `pts` (n,3) fp32 device points, n <= N:
         voxelise, stem + 4 stages + 4 ups through the fused conv kernels (one pass), head on voxel rows, slice back to the points.
+        batch_col (n,) fp32: the scan of every point (a batch engine refines the survivors of all its scans in one pass).
         Returns (n,18) fp32 offsets on the device."""
         if self.refine is None:
             raise RuntimeError("DenoiseEngine was built without the refinement network (sd_refine)")
-        h, g, N = self.h, self.geom, self.N
+        h, g, N = self.h, self.geom, self.cap
         pts = pts.to(device=self.device, dtype=torch.float32).contiguous()
         n = pts.shape[0]
         if n > N:
@@ -788,7 +807,7 @@ class DenoiseEngine:
         coords = self.buf("r.coords", (N, 4))
         q = self.buf("r.q", (N, 3))
         h.quantize(pts, self.resolution, self.div_mode, q[:n])
-        coords[:n, 0] = 0
+        coords[:n, 0] = 0 if batch_col is None else batch_col
         coords[:n, 1:] = q[:n]
         g.build(coords, n)
         F0 = self.act("r.F0", 1, N, 3)
@@ -812,3 +831,54 @@ class DenoiseEngine:
         if self.h.read_status() & 1:
             raise RuntimeError("lidiff_b200: a coordinate left the supported key range during sampling")
         return refined, post
+
+    def postprocess_batch(self, completed: torch.Tensor, x_init: torch.Tensor):
+        """postprocess() of every scan of a batch without a host synchronisation: completed (B*N,3) fp32, x_init (B,N,3) fp64 ->
+        (survivors (m,3) in scan order, their batch column (m,) fp32, survivors per scan (B,) int64), all on the device.  Each
+        scan's z band comes from the same reductions postprocess() runs (one strided column of N values each) and is compared in
+        fp32, as postprocess() compares with its host scalars."""
+        B, N = self.B, self.N
+        x, y, z = completed[:, 0], completed[:, 1], completed[:, 2]
+        dist = torch.sqrt((x * x + y * y) + z * z)
+        zi = x_init.reshape(B, N, 3)
+        max_z = torch.stack([zi[b, :, 2].max() for b in range(B)]).float()
+        min_z = torch.stack([zi[b, :, 2].mean() - 2 * zi[b, :, 2].std() for b in range(B)]).float()
+        keep = ((dist < self.max_range).reshape(B, N) & (z.reshape(B, N) < max_z[:, None]) & (z.reshape(B, N) > min_z[:, None])).reshape(-1)
+        return completed[keep].contiguous(), self._bcol[keep].contiguous(), keep.reshape(B, N).sum(1)
+
+    def complete_batch(self, x_init: torch.Tensor, x_feats: torch.Tensor, step_noise=None, fresh=True):
+        """complete() of the B scans of a batch engine: x_init / x_feats (B,N,3), step_noise (T,B,N,3) or None.  T denoising steps
+        for all scans at once, the batch's postprocess on the device, one refinement pass over the survivors of every scan.
+        Returns [(refined (6n_b,3), post (n_b,3))] per scan, device tensors."""
+        if self.B == 1:
+            return [self.complete(x_init, x_feats, step_noise, fresh=fresh)]
+        x_t = self.run(x_init, x_feats, step_noise, return_device=True, fresh=fresh)
+        post, bcol, counts = self.postprocess_batch(x_t, x_init.to(self.device))
+        off = self.refine_offsets(post, bcol).reshape(-1, 6, 3)
+        refined = (post[:, None, :] + off).reshape(-1, 3)
+        if self.h.read_status() & 1:
+            raise RuntimeError("lidiff_b200: a coordinate left the supported key range during sampling")
+        counts = counts.tolist()
+        return list(zip(refined.split([6 * c for c in counts]), post.split(counts)))
+
+
+# device bytes per point row of a whole completion with the engine: the peak of scripts/bench_batch.py on an H100 80GB HBM3 is
+# 117.1-117.8 KB at 180 000 points per scan (B = 1, 2, 3), plus a margin for the allocator's rounding
+ENGINE_BYTES_PER_ROW = 120_000
+MAX_BATCH = 1 << 10                  # coordinate keys carry 10 batch bits (csrc/common.cuh)
+
+
+def _check_batch(B: int, n_points: int, device):
+    """refuse, before any allocation, a batch whose batch column leaves the key range or whose buffers cannot fit"""
+    if not 1 <= B <= MAX_BATCH:
+        raise RuntimeError(f"DenoiseEngine: batch={B} is outside 1..{MAX_BATCH} (coordinate keys carry 10 batch bits)")
+    rows = B * n_points
+    if 27 * rows >= 1 << 31:
+        raise RuntimeError(f"DenoiseEngine: batch={B} x {n_points} points = {rows} rows exceed the 32-bit kernel-map index range")
+    if device.type == "cuda" and torch.cuda.is_available():
+        free, _ = torch.cuda.mem_get_info(device)
+        free += torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)     # cached by torch, free to reuse
+        need = rows * ENGINE_BYTES_PER_ROW
+        if need > free:
+            raise RuntimeError(f"DenoiseEngine: batch={B} x {n_points} points needs about {need / 2**30:.1f} GiB of device memory, "
+                               f"{free / 2**30:.1f} GiB are free")

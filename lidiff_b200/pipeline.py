@@ -14,6 +14,7 @@ drawn with torch.randn exactly where the reference draws it.
 from __future__ import annotations
 
 import copy
+import gc
 
 import numpy as np
 import torch
@@ -22,6 +23,10 @@ import torch.nn as nn
 from . import me as ME
 from . import minkunet as minknet
 from .scheduler import DPMSolverMultistepScheduler
+
+# batches of at least this many scans sample their points with the cluster kernel (all scans at once); smaller ones with the
+# single-scan kernel per scan, which is faster below that (scripts/bench_batch.py, DESIGN.md §3)
+FPS_CLUSTER_MIN_SCANS = 3
 
 DEFAULT_HPARAMS = {       # /root/reference/lidiff/config/config.yaml
     "data": {"resolution": 0.05, "num_points": 180000, "max_range": 50.0},
@@ -78,7 +83,8 @@ class DiffCompletion(nn.Module):
         hp["data"]["max_range"] = 50.0
         self.w_uncond = hp["train"]["uncond_w"]
         self.use_engine = engine
-        self._engine = None
+        self._engine = None              # the one fused engine alive, sized for the batch size in use
+        self._last_batch = 1             # batch size of the last trajectory (a different one starts fresh)
 
     device = property(lambda self: self._device)
 
@@ -110,6 +116,22 @@ class DiffCompletion(nn.Module):
         sel = farthest_point_sample(pts, int(self.hparams["data"]["num_points"] / 10))
         return pts[sel].repeat(10, 1)[None, :, :]
 
+    def preprocess_scans(self, scans):
+        """preprocess_scan of every scan, the farthest point sampling of all of them in one launch -> (B, num_points, 3) fp64"""
+        from .preprocess import farthest_point_sample, farthest_point_sample_batched
+        pts = []
+        for scan in scans:
+            scan = np.asarray(scan)
+            dist = np.sqrt(np.sum(scan ** 2, -1))
+            pts.append(torch.as_tensor(scan[(dist < self.hparams["data"]["max_range"]) & (dist > 3.5)][:, :3], dtype=torch.float64,
+                                       device=self.device))
+        n_s = int(self.hparams["data"]["num_points"] / 10)
+        if len(pts) >= FPS_CLUSTER_MIN_SCANS:
+            sel = farthest_point_sample_batched(pts, n_s)
+        else:
+            sel = [farthest_point_sample(p, n_s) for p in pts]
+        return torch.stack([p[s].repeat(10, 1) for p, s in zip(pts, sel)])
+
     def postprocess_scan(self, completed_scan, input_scan):
         dist = np.sqrt(np.sum(completed_scan ** 2, -1))
         post_scan = completed_scan[dist < self.hparams["data"]["max_range"]]
@@ -122,6 +144,8 @@ class DiffCompletion(nn.Module):
         """fresh=False (default) keeps the scheduler's multistep state between scans like the reference does (its main loop,
         :213-222, never calls set_timesteps again: the first update of every scan after the first is second-order against the
         previous scan's last x0); fresh=True starts a new trajectory."""
+        fresh = fresh or self._last_batch != 1      # after a batch of another size the multistep state does not fit this scan
+        self._last_batch = 1
         scan = scan if preprocessed else self.preprocess_scan(scan)
         scan = scan.to(self.device)
         if start_noise is None:
@@ -139,6 +163,59 @@ class DiffCompletion(nn.Module):
         offset = self.refine_forward(refine_in).reshape(-1, 6, 3)
         refine_complete_scan = post_scan[:, None, :] + offset.cpu().numpy()
         return refine_complete_scan.reshape(-1, 3), post_scan
+
+    def complete_scans(self, scans, start_noise=None, step_noise=None, preprocessed=False, fresh=False):
+        """complete_scan of B scans that share every launch: one trajectory per scan in batch column b, as the reference's
+        batched p_sample_loop (lidiff/models/models.py:132-151) samples them.  start_noise (B,N,3), step_noise (T,B,N,3); by
+        default the noise is drawn once per step with shape (B,N,3).  Returns [(refined, post)] per scan, each what
+        complete_scan(scans[b], start_noise[b], step_noise[:, b], fresh=True) gives up to the fp32 rounding of the sparse
+        convolutions, which depends on the rows that share a tile (DESIGN.md §3, batched sampling).  fresh=False carries every slot's multistep
+        state into the next batch of the same size; a batch of another size (a short last batch) starts fresh."""
+        B = len(scans)
+        fresh = fresh or B != self._last_batch
+        if B == 1:
+            r = self.complete_scan(scans[0], None if start_noise is None else start_noise[0:1],
+                                   None if step_noise is None else step_noise[:, 0], preprocessed=preprocessed, fresh=fresh)
+            return [r]
+        self._last_batch = B
+        x_init = (torch.stack([torch.as_tensor(s).reshape(-1, 3) for s in scans]) if preprocessed else self.preprocess_scans(scans))
+        x_init = x_init.to(self.device)
+        if start_noise is None:
+            start_noise = torch.randn(x_init.shape, device=self.device)
+        x_feats = x_init + start_noise.to(self.device)
+        if self.use_engine:
+            outs = self.engine(B).complete_batch(x_init, x_feats, step_noise, fresh=fresh)
+            return [(r.cpu().numpy(), p.cpu().numpy()) for r, p in outs]
+        x_full = self.points_to_tensor(x_feats)
+        x_cond = self.points_to_tensor(x_init)
+        x_uncond = self.points_to_tensor(torch.zeros_like(x_init))
+        completed = self.completion_loop_batch(x_init, x_full, x_cond, x_uncond, step_noise, fresh=fresh).reshape(B, -1, 3)
+        posts = [self.postprocess_scan(completed[b], x_init[b]) for b in range(B)]
+        refine_in = self.points_to_tensor([torch.as_tensor(p) for p in posts])
+        offset = self.refine_forward(refine_in).reshape(-1, 6, 3).cpu().numpy()
+        out, k = [], 0
+        for p in posts:
+            out.append(((p[:, None, :] + offset[k:k + p.shape[0]]).reshape(-1, 3), p))
+            k += p.shape[0]
+        return out
+
+    def completion_loop_batch(self, x_init, x_t, x_cond, x_uncond, step_noise=None, fresh=False):
+        """completion_loop over B scans in one TensorField (x_init (B,N,3)), as the reference's p_sample_loop runs it: the
+        timestep repeated per scan, one scheduler step over (B,N,3)"""
+        self.scheduler_to_cuda()
+        if fresh:
+            self.dpm_scheduler.set_timesteps(self.dpm_scheduler.num_inference_steps, device=self.device)
+        B = x_init.shape[0]
+        for i in range(len(self.dpm_scheduler.timesteps)):
+            t = torch.ones(B, dtype=torch.long, device=self.device) * self.dpm_scheduler.timesteps[i]
+            noise_t = self.classfree_forward(x_t, x_cond, x_uncond, t)
+            input_noise = x_t.F.reshape(B, -1, 3) - x_init
+            nz = None if step_noise is None else step_noise[i].to(self.device)
+            x_t = x_init + self.dpm_scheduler.step(noise_t, t[0], input_noise, noise=nz)["prev_sample"]
+            x_t = self.points_to_tensor(x_t)
+            x_cond = self.points_to_tensor(x_cond.F.reshape(B, -1, 3).detach())
+            x_uncond = self.points_to_tensor(torch.zeros_like(x_cond.F.reshape(B, -1, 3)))
+        return x_t.F.cpu().detach().numpy()
 
     def refine_forward(self, x_in):
         with torch.no_grad():
@@ -173,8 +250,16 @@ class DiffCompletion(nn.Module):
         return x_t.F.cpu().detach().numpy()
 
     # ---- fused path -----------------------------------------------------------------------------------
-    def engine(self):
+    def engine(self, batch=1):
+        """the fused engine for batches of `batch` scans.  An engine holds its buffers and step graphs for one batch size (about
+        20 GiB per 180 000-point scan), so one is alive at a time: asking for another batch size (a short last batch) releases
+        the current engine and returns its memory to the device before the new one is sized."""
+        if self._engine is not None and self._engine.B != batch:
+            self._engine = None
+            gc.collect()
+            if torch.cuda.is_available():
+                torch.cuda.empty_cache()
         if self._engine is None:
             from .engine import DenoiseEngine
-            self._engine = DenoiseEngine.from_modules(self)
+            self._engine = DenoiseEngine.from_modules(self, **({} if batch == 1 else {"batch": batch}))
         return self._engine

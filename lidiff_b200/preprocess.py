@@ -24,3 +24,29 @@ def farthest_point_sample(points: torch.Tensor, n_samples: int, ordered: bool = 
     h.farthest_point_sample(pts, n, n_samples, idx, dist)
     idx = idx.long()
     return torch.sort(idx).values if ordered else idx
+
+
+def farthest_point_sample_batched(scans: list[torch.Tensor], n_samples: int, ordered: bool = True) -> torch.Tensor:
+    """`farthest_point_sample` of every scan of `scans` (CUDA (n_b, 3) tensors of any sizes >= n_samples) in one launch of the
+    cluster kernel: (B, n_samples) int64 scan-local indices, each row equal to farthest_point_sample(scans[b], n_samples).
+    Scans larger than the kernel's on-chip capacity are sampled one by one with the single-scan kernel."""
+    if not all(s.is_cuda for s in scans):
+        raise RuntimeError("farthest_point_sample_batched: CUDA tensors required (no CPU fallback)")
+    sizes = [int(s.shape[0]) for s in scans]
+    if not scans or min(sizes) < n_samples:
+        raise RuntimeError(f"farthest_point_sample_batched: asked for {n_samples} of {min(sizes, default=0)} points")
+    dev = scans[0].device
+    h = _lib.get_handle(dev)
+    out = torch.empty((len(scans), n_samples), dtype=torch.int64, device=dev)
+    cap = h.fps_batched_capacity()
+    on_chip = [b for b, n in enumerate(sizes) if n <= cap]
+    for b in range(len(scans)):
+        if b not in on_chip:
+            out[b] = farthest_point_sample(scans[b], n_samples, ordered=False)
+    if on_chip:
+        pts = torch.cat([scans[b].to(torch.float64).reshape(-1, 3) for b in on_chip]).contiguous()
+        offsets = torch.tensor([0] + [sizes[b] for b in on_chip], dtype=torch.int64).cumsum(0).to(dev)
+        idx = torch.empty((len(on_chip), n_samples), dtype=torch.int32, device=dev)
+        h.farthest_point_sample_batched(pts, offsets, len(on_chip), max(sizes[b] for b in on_chip), n_samples, idx)
+        out[on_chip] = idx.long()
+    return torch.sort(out, dim=1).values if ordered else out

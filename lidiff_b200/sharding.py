@@ -16,6 +16,14 @@ def scans_of_rank(n_scans: int, world: int, rank: int) -> list[int]:
     return [b for b in range(n_scans) if b % world == rank]
 
 
+def batches_of_rank(n_scans: int, world: int, rank: int, batch: int) -> list[list[int]]:
+    """the scans of this rank (scans_of_rank) in groups of `batch`, in order; the last group may be shorter"""
+    if batch < 1:
+        raise ValueError(f"batch size must be >= 1, got {batch}")
+    mine = scans_of_rank(n_scans, world, rank)
+    return [mine[i:i + batch] for i in range(0, len(mine), batch)]
+
+
 def max_over_ranks(ms: float, device) -> float:
     """the job's time is the slowest rank's device time"""
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:

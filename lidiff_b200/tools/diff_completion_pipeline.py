@@ -3,7 +3,8 @@
 (/root/reference/lidiff/tools/diff_completion_pipeline.py:179-212): same options, same outputs
 (`results/<exp>/{diff,refine}/<scan>.ply`; with `--normals` each PLY also carries the reference's open3d estimate_normals()
 normals as `nx ny nz`, computed on the GPU by lidiff_b200.normals), plus sharding of the scans over the ranks of a torchrun job
-(one process per GPU, scan b on rank b mod R; SURVEY.md 8e).
+(one process per GPU, scan b on rank b mod R; SURVEY.md 8e).  --batch-size B completes a rank's scans B at a time
+(DiffCompletion.complete_scans: one trajectory per scan, every launch shared); the files written are the same as with B = 1.
 
     torchrun --nproc-per-node 8 -m lidiff_b200.tools.diff_completion_pipeline -d diff.ckpt -r refine.ckpt --path ./Datasets/test
     python -m lidiff_b200.tools.diff_completion_pipeline --random-weights --path ./Datasets/test     # no checkpoints at hand
@@ -19,7 +20,7 @@ import torch
 
 from ..normals import estimate_normals
 from ..pipeline import DiffCompletion
-from ..sharding import scans_of_rank
+from ..sharding import batches_of_rank
 from ..synth import read_ply_xyz
 
 
@@ -56,7 +57,8 @@ def write_ply(path: str, pts: np.ndarray, normals: np.ndarray | None = None):
 @click.option("--out", type=str, default="./results", help="output root")
 @click.option("--random-weights", is_flag=True, help="seeded random parameters instead of checkpoints (plumbing / benchmarking)")
 @click.option("--normals", is_flag=True, help="write open3d's estimate_normals() (30 nearest neighbours) as nx ny nz, as the reference does")
-def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, normals):
+@click.option("--batch-size", type=click.IntRange(min=1), default=1, help="scans completed together per denoising loop (default: 1)")
+def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, normals, batch_size):
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
     device = torch.device("cuda", local_rank)
@@ -74,17 +76,18 @@ def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, 
     os.makedirs(f"{out}/{exp_dir}/refine", exist_ok=True)
     os.makedirs(f"{out}/{exp_dir}/diff", exist_ok=True)
     files = sorted(os.listdir(path), key=lambda s: [int(t) if t.isdigit() else t for t in __import__("re").split(r"(\d+)", s)])
-    mine = [files[i] for i in scans_of_rank(len(files), world, rank)]
-    for name in mine:
-        points = load_pcd(os.path.join(path, name))
+    for group in batches_of_rank(len(files), world, rank, batch_size):
+        names = [files[i] for i in group]
+        points = [load_pcd(os.path.join(path, name)) for name in names]
         start = time.time()
-        refine_scan, diff_scan = pipe.complete_scan(points)
+        results = [pipe.complete_scan(points[0])] if batch_size == 1 else pipe.complete_scans(points)
         torch.cuda.synchronize()
-        print(f"[rank {rank}] {name}: took {time.time() - start:.3f}s")
-        stem = name.split(".")[0]
-        for kind, cloud in (("refine", refine_scan), ("diff", diff_scan)):
-            nrm = estimate_normals(cloud, device=device).cpu().numpy() if normals else None
-            write_ply(f"{out}/{exp_dir}/{kind}/{stem}.ply", cloud, nrm)
+        print(f"[rank {rank}] {', '.join(names)}: took {time.time() - start:.3f}s")
+        for name, (refine_scan, diff_scan) in zip(names, results):
+            stem = name.split(".")[0]
+            for kind, cloud in (("refine", refine_scan), ("diff", diff_scan)):
+                nrm = estimate_normals(cloud, device=device).cpu().numpy() if normals else None
+                write_ply(f"{out}/{exp_dir}/{kind}/{stem}.ply", cloud, nrm)
     if world > 1:
         import torch.distributed as dist
         dist.barrier()

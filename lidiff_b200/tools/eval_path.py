@@ -9,7 +9,8 @@ cd_mean, cd_std, pr, re, f1) next to --path, with every metric computed on the G
 Two modes: with -d / -r (or --random-weights) every scan is completed with lidiff_b200.pipeline.DiffCompletion and the refined
 cloud is scored (--cloud diff scores the diffusion-only cloud); without them the `<stem>.ply` files in --path are scored, as
 lidiff_b200.tools.diff_completion_pipeline writes them.  Under torchrun scan b runs on rank b mod R; rank 0 folds the per-scan
-records in scan order, so the results do not depend on the number of ranks.
+records in scan order, so the results do not depend on the number of ranks.  --batch-size B completes a rank's scans B at a
+time (DiffCompletion.complete_scans); res_log.yaml has the same layout as with B = 1.
 """
 from __future__ import annotations
 
@@ -22,7 +23,7 @@ import torch
 
 from .. import metrics as M
 from ..kitti import load_poses, natural_sorted, parse_calibration  # noqa: F401  (part of this module's interface)
-from ..sharding import gather_scans, scans_of_rank
+from ..sharding import batches_of_rank, gather_scans
 from ..shims.open3d.geometry import PointCloud, VoxelGrid
 from ..synth import read_ply_xyz
 
@@ -41,29 +42,34 @@ def ground_truth(pose: np.ndarray, cur_scan: np.ndarray, seq_map: np.ndarray, ma
 
 def scan_completion(data: str, scan_name: str, path: str, pipe, max_range: float, cloud: str):
     """(prediction, the scan's points within max_range)"""
-    points = np.fromfile(os.path.join(data, "velodyne", scan_name), dtype=np.float32).reshape(-1, 4)
-    dist = np.sqrt(np.sum(points[:, :3] ** 2, axis=-1))
-    cur = points[dist < max_range, :3]
+    return scan_completions(data, [scan_name], path, pipe, max_range, cloud)[0]
+
+
+def scan_completions(data: str, scan_names: list, path: str, pipe, max_range: float, cloud: str, batched: bool = False):
+    """[(prediction, the scan's points within max_range)] of a group of scans; batched: completed by complete_scans (one
+    trajectory per scan, a group shorter than the others starts fresh), else one by one by complete_scan"""
+    points = [np.fromfile(os.path.join(data, "velodyne", s), dtype=np.float32).reshape(-1, 4) for s in scan_names]
+    curs = [p[np.sqrt(np.sum(p[:, :3] ** 2, axis=-1)) < max_range, :3] for p in points]
     if pipe is None:
-        pred = read_ply_xyz(os.path.join(path, f"{scan_name.split('.')[0]}.ply"))
-        pred = pred[np.sqrt(np.sum(pred ** 2, axis=-1)) < max_range]
+        preds = [read_ply_xyz(os.path.join(path, f"{s.split('.')[0]}.ply")) for s in scan_names]
+        preds = [p[np.sqrt(np.sum(p ** 2, axis=-1)) < max_range] for p in preds]
     else:
-        refined, diff = pipe.complete_scan(points)
-        pred = refined if cloud == "refine" else diff
-    return pred, cur
+        done = pipe.complete_scans(points) if batched else [pipe.complete_scan(p) for p in points]
+        preds = [refined if cloud == "refine" else diff for refined, diff in done]
+    return list(zip(preds, curs))
 
 
-def score_scans(data: str, path: str, pipe, max_range: float, cloud: str, device, rank: int = 0, world: int = 1):
-    """(number of scans, {scan index: record as rows}) for the scans of this rank"""
+def score_scans(data: str, path: str, pipe, max_range: float, cloud: str, device, rank: int = 0, world: int = 1, batch: int = 1):
+    """(number of scans, {scan index: record as rows}) for the scans of this rank, completed `batch` at a time"""
     poses = load_poses(os.path.join(data, "calib.txt"), os.path.join(data, "poses.txt"))
     seq_map = np.load(os.path.join(data, "map_clean.npy"))
     scans = natural_sorted(os.listdir(os.path.join(data, "velodyne")))
     n = min(len(poses), len(scans))
     local = {}
-    for b in scans_of_rank(n, world, rank):
-        pred, cur = scan_completion(data, scans[b], path, pipe, max_range, cloud)
-        gt = ground_truth(poses[b], cur, seq_map, max_range)
-        local[b] = M.record_to_rows(M.evaluate_scan(gt, pred, device=device))
+    for group in batches_of_rank(n, world, rank, batch):
+        for b, (pred, cur) in zip(group, scan_completions(data, [scans[b] for b in group], path, pipe, max_range, cloud, batch > 1)):
+            gt = ground_truth(poses[b], cur, seq_map, max_range)
+            local[b] = M.record_to_rows(M.evaluate_scan(gt, pred, device=device))
     return n, local
 
 
@@ -123,7 +129,8 @@ def log_path(path: str) -> str:
 @click.option("--random-weights", is_flag=True, help="complete with seeded random parameters instead of checkpoints (plumbing)")
 @click.option("--data", type=str, default=PATH_DATA, help="sequence directory: velodyne/*.bin, calib.txt, poses.txt, map_clean.npy")
 @click.option("--cloud", type=click.Choice(["refine", "diff"]), default="refine", help="which completed cloud to score")
-def main(path, voxel_size, max_range, denoising_steps, cond_weight, diff, refine, random_weights, data, cloud):
+@click.option("--batch-size", type=click.IntRange(min=1), default=1, help="scans completed together per denoising loop (default: 1)")
+def main(path, voxel_size, max_range, denoising_steps, cond_weight, diff, refine, random_weights, data, cloud, batch_size):
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(device)
@@ -139,7 +146,7 @@ def main(path, voxel_size, max_range, denoising_steps, cond_weight, diff, refine
     elif diff is not None or refine is not None:
         from ..pipeline import DiffCompletion
         pipe = DiffCompletion(diff, refine, denoising_steps, cond_weight, device=device)
-    n, local = score_scans(data, path, pipe, max_range, cloud, device, rank, world)
+    n, local = score_scans(data, path, pipe, max_range, cloud, device, rank, world, batch_size)
     gathered = gather_scans(local, n, device)
     if rank == 0:
         res = fold({b: M.record_from_rows(rows) for b, rows in gathered.items()})
