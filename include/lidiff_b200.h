@@ -46,13 +46,17 @@ int         lb2_version(void);
 /* number of kernels this library has launched through `handle` since creation (bench gpu_launches) */
 int64_t     lb2_launch_count(void* handle);
 /* synchronising read-and-clear of the device status word; bit0 = a coordinate fell outside the key
- * range (10 bit batch, 18 bit signed axes) and was clamped.  Returns the word (>= 0) or an error. */
+ * range (batch in [0, 1023], every axis in [-131072, 131071]) or was NaN, and its key was clamped into
+ * the range.  Returns the word (>= 0) or an error. */
 int         lb2_read_status(void* handle, void* stream);
 
 /* ---- hash grid (coordinate manager)  — replaces ME's CoordinateManager -------------------------
  * One hash grid per coordinate level.  `keys` (uint64[cap_table]) and `vals` (int32[2*cap_table]:
  * [0,cap) scratch "first point index", [cap,2cap) row id) are caller-owned; cap_table is a power
- * of two >= 2 * max rows.  Key packing: 10 bit batch | 3 x 18 bit signed coordinate.
+ * of two >= 2 * max rows.  Key packing: 10 bit batch | 3 x 18 bit signed coordinate, so the key range is
+ * batch in [0, 1023] and every axis in [-131072, 131071].  The range is closed under the stride maps' floor
+ * to multiples of 2^l: a level-0 row in range has every coarser row in range.  A kernel-map neighbour outside
+ * the range is a miss (nothing wraps).
  */
 typedef struct {
     uint64_t* keys;
@@ -71,7 +75,11 @@ int lb2_quantize(void* h, void* stream, const float* x, int64_t n_elem, float re
  * Input rows: either fp32 integer-valued coords (`in_f`, floor() is applied; TensorField) or int32
  * coords (`in_i`; a parent level).  If ts_floor > 0 the xyz columns are floored to multiples of
  * ts_floor (stride map).  Output: unique rows in FIRST-OCCURRENCE order, `inverse[i]` = output row of
- * input row i, `*d_nout` = number of unique rows.  `scratch` >= lb2_unique_scratch_bytes(n_cap). */
+ * input row i, `*d_nout` = number of unique rows.  `scratch` >= lb2_unique_scratch_bytes(n_cap).
+ * n_cap <= 4194304 (4M rows; larger: LB2_ERR_ARG).  Rows past min(*d_nin, n_cap) are not read.
+ * Non-finite in_f values: +-inf and values beyond the int32 range convert to INT_MIN / INT_MAX, NaN to 0; such a
+ * row (a NaN in any column, or any column outside the key range) raises status bit 0 (lb2_read_status) and is
+ * grouped under its clamped key, so the caller must treat the build as failed. */
 size_t lb2_unique_scratch_bytes(int64_t n_cap);
 int lb2_unique_build(void* h, void* stream,
                      const float* in_f, const int32_t* in_i, const int32_t* d_nin, int32_t n_cap,
@@ -79,8 +87,14 @@ int lb2_unique_build(void* h, void* stream,
                      int32_t* out_coords, int32_t* inverse, int32_t* d_nout, void* scratch);
 
 /* UNWEIGHTED_AVERAGE voxel features (ME.SparseTensorQuantizationMode, pipeline:77): mean of member
- * point features, out (m_cap, c).  The sums are exact fixed-point sums (2^-61 of the largest member magnitude), so the result
- * does not depend on the order of the points.  `scratch` >= lb2_voxel_mean_scratch_bytes(m_cap, c) bytes. */
+ * point features, out (m_cap, c).  Every member is rounded to a fixed-point quantum 2^-s and summed exactly in int64, so the
+ * result does not depend on the order of the points.  For a (row, channel) with n members, largest magnitude in
+ * [2^(e-1), 2^e), s = 61 - e - bitlen(n) and exact mean m:
+ *     |out - m| <= ulp32(m)/2 + 2^-(s+1) + 2^-50 |m|,
+ * and out = RN32(m) wherever m is farther than 2^-(s+1) + 2^-50 |m| from an fp32 rounding midpoint (2^-(s+1) is about
+ * 2^-51 of the largest member for a 1000-member voxel).  Rows whose members are all zero are +0; a row with a NaN or +-inf
+ * member is NaN in that channel (ME's fp32 sum would give +-inf for an inf member), as is a row with no members;
+ * rows [*d_m, m_cap) are 0.  `scratch` >= lb2_voxel_mean_scratch_bytes(m_cap, c) bytes. */
 size_t lb2_voxel_mean_scratch_bytes(int32_t m_cap, int32_t c);
 int lb2_voxel_mean(void* h, void* stream, const float* feats, const int32_t* inverse, int32_t n,
                    int32_t c, const int32_t* d_m, int32_t m_cap, float* out, void* scratch);
@@ -107,7 +121,8 @@ int lb2_kernel_map_self(void* h, void* stream, lb2_grid grid, const int32_t* coo
  * Results do not depend on the order.  scratch >= lb2_row_order_scratch_bytes(n_cap).
  * coords (optional, kvol 27 only): the rows' int32 [b,x,y,z] coordinates; rows of equal mask are then ordered by the Morton code of
  * (x,y,z) >> coord_shift (coord_shift = log2 of the level's tensor stride), which makes the tiles of large mask groups spatially
- * compact (L2 locality of the gathers). */
+ * compact (L2 locality of the gathers).  The sort is stable: rows of equal key (and Morton code) keep their index order, so
+ * the order, and with it the tensor-core convolution's per-tile accumulation grouping, is the same on every run. */
 size_t lb2_row_order_scratch_bytes(int32_t n_cap);
 int lb2_row_order(void* h, void* stream, const uint32_t* row_mask, const int32_t* d_n, int32_t n_cap,
                   int32_t kvol, int32_t* perm, void* scratch, const int32_t* coords, int32_t coord_shift);

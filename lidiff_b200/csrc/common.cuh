@@ -51,12 +51,15 @@ int rs_sort_keys(Lb2Handle* h, cudaStream_t s, const unsigned* keys, const int* 
 
 // ---------------------------------------------------------------------------------------------------
 // coordinate keys: 10 bit batch | 3 x 18 bit biased coordinate  (same packing as oracle/me_cpu.py)
+// Key range: batch in [0, 1023], every axis in [-131072, 131071] (18-bit two's complement).  The range is closed under the
+// stride maps' floor to a multiple of 2^l (-2^17 is such a multiple), so a level-0 row in range has every coarser row in range.
 // ---------------------------------------------------------------------------------------------------
 #define LB2_AXIS_BITS 18
 #define LB2_AXIS_OFF  (1 << (LB2_AXIS_BITS - 1))
 
 __device__ __forceinline__ bool lb2_pack_key(int b, int x, int y, int z, unsigned long long& key) {
-    unsigned ux = (unsigned)(x + LB2_AXIS_OFF), uy = (unsigned)(y + LB2_AXIS_OFF), uz = (unsigned)(z + LB2_AXIS_OFF);
+    // biased in unsigned arithmetic: the saturated conversions of +-inf (INT_MAX / INT_MIN) wrap instead of overflowing
+    unsigned ux = (unsigned)x + LB2_AXIS_OFF, uy = (unsigned)y + LB2_AXIS_OFF, uz = (unsigned)z + LB2_AXIS_OFF;
     const unsigned lim = 1u << LB2_AXIS_BITS;
     bool ok = ((unsigned)b < 1024u) && ux < lim && uy < lim && uz < lim;
     if (!ok) {   // keep memory-safe: clamp; caller raises the status bit

@@ -110,11 +110,14 @@ __global__ void k_grid_clear(unsigned long long* keys, int* vals, int cap) {
     if (i < cap) { keys[i] = LB2_KEY_EMPTY; vals[i] = INT_MAX; vals[cap + i] = -1; }
 }
 
-__device__ __forceinline__ int4 load_row(const float* __restrict__ in_f, const int* __restrict__ in_i, int i, int ts) {
+// fp32 rows: floor, then the conversion saturates (+-inf and huge values land outside the key range) and turns NaN into 0,
+// so `nan` reports a NaN component: such a row is outside the key range too
+__device__ __forceinline__ int4 load_row(const float* __restrict__ in_f, const int* __restrict__ in_i, int i, int ts, bool* nan = nullptr) {
     int4 c;
     if (in_f) {
         float4 f = __ldg(reinterpret_cast<const float4*>(in_f) + i);
         c = make_int4((int)floorf(f.x), (int)floorf(f.y), (int)floorf(f.z), (int)floorf(f.w));
+        if (nan) *nan = isnan(f.x) || isnan(f.y) || isnan(f.z) || isnan(f.w);
     } else {
         c = __ldg(reinterpret_cast<const int4*>(in_i) + i);
     }
@@ -129,9 +132,10 @@ __global__ void k_grid_insert(const float* __restrict__ in_f, const int* __restr
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     int n = d_n ? min(*d_n, n_cap) : n_cap;
     if (i >= n) return;
-    int4 c = load_row(in_f, in_i, i, ts);
+    bool nan = false;
+    int4 c = load_row(in_f, in_i, i, ts, &nan);
     unsigned long long key;
-    if (!lb2_pack_key(c.x, c.y, c.z, c.w, key)) atomicOr(status, 1);
+    if (!lb2_pack_key(c.x, c.y, c.z, c.w, key) || nan) atomicOr(status, 1);
     unsigned slot = lb2_hash(key) & mask;
     while (true) {
         unsigned long long prev = atomicCAS(keys + slot, (unsigned long long)LB2_KEY_EMPTY, key);
@@ -270,7 +274,9 @@ extern "C" int lb2_unique_build(void* handle, void* stream, const float* in_f, c
 // The sums are exact and independent of the order in which points arrive: each (voxel, channel) sum is accumulated in int64 fixed point
 // at a scale set by the largest member magnitude and the member count (every value v becomes round(v * 2^s) with |sum| < 2^61), then
 // divided by the count in fp64 and rounded once to fp32.  fp32 atomics would make the last bits, and through the re-voxelisation of the
-// next steps whole trajectories, differ from run to run.
+// next steps whole trajectories, differ from run to run.  Error (n members, 2^(e-1) <= largest |member| < 2^e, s = 61 - e - bitlen(n),
+// m the exact mean): |out - m| <= ulp32(m)/2 + 2^-(s+1) + 2^-50 |m|, the middle term from rounding every member to 2^-s, the last from
+// the fp64 conversion and division.  A NaN or +-inf member makes the mean NaN.
 __device__ __forceinline__ int voxel_fix_shift(float maxabs, int count) {
     int e;
     frexpf(maxabs, &e);                                   // maxabs < 2^e

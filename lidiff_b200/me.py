@@ -70,7 +70,8 @@ class CoordinateManager:
         # only the level-0 insertion can leave the key range (coarser levels floor coordinates that are already in range): one status
         # read per TensorField, right behind the build that could have raised it (the word is per device and cleared by the read)
         if ts_floor == 0 and (h.read_status() & 1):
-            raise RuntimeError("lidiff_b200.me: coordinate outside the supported key range (|x| < 131072 voxels, batch < 1024)")
+            raise RuntimeError("lidiff_b200.me: coordinate outside the supported key range "
+                               "(-131072 <= x <= 131071 voxels, 0 <= batch < 1024, no NaN)")
         return _Level(out[:n], n, d_n, grid, inv)
 
     def insert_field(self, coords_f: torch.Tensor):

@@ -14,19 +14,25 @@ import torch
 
 # ----------------------------------------------------------------------------------------------
 # coordinate packing: [b | x | y | z] -> one int64 so numpy can unique / searchsorted on it.
-# 10 bits batch (0..1023), 18 bits signed per axis (+-131072 voxels = +-6.5 km at 5 cm).
-# The CUDA hash grid uses the same packing (lidiff_b200/csrc/coords.cuh).
+# 10 bits batch (0..1023), 18 bits two's complement per axis: [-131072, 131071] voxels (+-6.5 km at
+# 5 cm), a range the stride levels' floor to multiples of 2^l never leaves.
+# The CUDA hash grid uses the same packing (lidiff_b200/csrc/common.cuh).
 # ----------------------------------------------------------------------------------------------
 AXIS_BITS = 18
 AXIS_OFF = 1 << (AXIS_BITS - 1)
 BATCH_MAX = 1 << 10
 
 
+def in_key_range(xyz: np.ndarray) -> np.ndarray:
+    """(..., 3) integer axes -> bool (...): every axis in [-AXIS_OFF, AXIS_OFF)"""
+    return ((xyz >= -AXIS_OFF) & (xyz < AXIS_OFF)).all(-1)
+
+
 def pack_keys(C: np.ndarray) -> np.ndarray:
     C = np.asarray(C, dtype=np.int64)
     if C.shape[0]:
         assert C[:, 0].min() >= 0 and C[:, 0].max() < BATCH_MAX, "batch index out of key range"
-        assert np.abs(C[:, 1:]).max() < AXIS_OFF, "coordinate out of key range"
+        assert in_key_range(C[:, 1:]).all(), "coordinate out of key range"
     return ((C[:, 0] << (3 * AXIS_BITS))
             | ((C[:, 1] + AXIS_OFF) << (2 * AXIS_BITS))
             | ((C[:, 2] + AXIS_OFF) << AXIS_BITS)
@@ -150,7 +156,7 @@ class Geometry:
             for off in self.kernel_offsets(ks, ts_in):
                 q = C_out.copy()
                 q[:, 1:] += off[None, :]
-                ok = (np.abs(q[:, 1:]) < AXIS_OFF).all(1)
+                ok = in_key_range(q[:, 1:])
                 qk = pack_keys(np.where(ok[:, None], q, 0))
                 pos = np.searchsorted(sorted_keys, qk)
                 pos = np.minimum(pos, sorted_keys.shape[0] - 1)

@@ -8,6 +8,7 @@ import ctypes as C
 import numpy as np
 import torch
 
+import coords_reference as cref
 from oracle import me_cpu as ome
 from split_numerics import split
 
@@ -86,8 +87,16 @@ class FakeHandle:
     def unique_build(self, in_f, in_i, d_nin, n_cap, ts_floor, grid, out_coords, inverse, d_nout, scratch):
         self.launches += 6
         n = self._n(d_nin, n_cap)
-        rows = torch.floor(in_f[:n]).long().numpy() if in_f is not None else in_i[:n].long().numpy()
-        rows = rows.copy()
+        if in_f is not None:
+            f = in_f[:n].numpy()
+            rows, bad = cref.floor_rows(f), cref.flagged(in_f=f)
+        else:
+            rows = in_i[:n].long().numpy().copy()
+            bad = cref.flagged(in_i=rows)
+        if bad.any():                              # status bit 0; the keys of such rows are clamped into the range, as on the GPU
+            self.status |= 1
+            rows[:, 0] = np.clip(rows[:, 0], 0, cref.BATCH_MAX)
+            rows[:, 1:] = np.clip(rows[:, 1:], cref.AXIS_MIN, cref.AXIS_MAX)
         if ts_floor > 0:
             rows[:, 1:] = np.floor_divide(rows[:, 1:], ts_floor) * ts_floor
         first, inv = ome.unique_first_occurrence(rows)
@@ -123,7 +132,7 @@ class FakeHandle:
         for k, off in enumerate(offs * step):
             q = Cq.copy()
             q[:, 1:] += off[None, :]
-            ok = (np.abs(q[:, 1:]) < ome.AXIS_OFF).all(1)
+            ok = ome.in_key_range(q[:, 1:])
             qk = ome.pack_keys(np.where(ok[:, None], q, 0))
             pos = np.minimum(np.searchsorted(skeys, qk), max(skeys.shape[0] - 1, 0))
             hit = ok & (skeys[pos] == qk) if skeys.shape[0] else np.zeros(n, bool)
