@@ -136,6 +136,19 @@ int lb2_row_order(void* h, void* stream, const uint32_t* row_mask, const int32_t
 int lb2_tile_order(void* h, void* stream, const uint32_t* row_mask, const int32_t* row_perm, const int32_t* d_n, int32_t n_cap,
                    int32_t* order128, int32_t* order256, void* scratch);
 
+/* Row and tile order of one offset range [k0, k1) of a kvol-27 map (0 <= k0 < k1 <= 27), for a convolution run as one launch per
+ * range (lb2_conv_desc.k0 / k1).  With sub = row_mask & bits [k0, k1): perm[0..n) = the rows sorted by the stable LSD radix sort
+ * of lb2_row_order on the key [sub == 0 | 2 or more bits of sub besides the centre (13) | sub without the centre bit], i.e. the rows
+ * with an empty sub-mask last and the others grouped by their sub-mask; *d_live (device int32) = the number of rows with a non-empty
+ * sub-mask.  No host synchronisation.  scratch >= lb2_row_order_scratch_bytes(n_cap). */
+int lb2_row_order_range(void* h, void* stream, const uint32_t* row_mask, const int32_t* d_n, int32_t n_cap, int32_t k0, int32_t k1,
+                        int32_t* perm, int32_t* d_live, void* scratch);
+
+/* lb2_tile_order for a range launch: order128 over the first cdiv(*d_n, 128) tiles of perm, cost = popcount of the OR of the
+ * tile's row masks restricted to [k0, k1).  Pass d_live for a range that is not the last, the map's row count for the last. */
+int lb2_tile_order_range(void* h, void* stream, const uint32_t* row_mask, const int32_t* row_perm, const int32_t* d_n, int32_t n_cap,
+                         int32_t k0, int32_t k1, int32_t* order128, void* scratch);
+
 /* ---- sparse convolution  — replaces ME.MinkowskiConvolution(+Transpose) forward, with the
  * MinkowskiBatchNorm(eval)/MinkowskiReLU/residual-add/ME.cat/gate-multiply that follow it in
  * minkunet.py:13-80,431,464 fused as prologue/epilogue.
@@ -191,6 +204,18 @@ typedef struct {
                                       persistent CTAs (heaviest first); ignored when nbr is NULL.  Scheduling only: results do not
                                       depend on it */
     const int32_t* tile_order256;  /* not read by this build */
+    /* Offset range (tensor-core variant only): with k1 > 0 the launch runs the kernel offsets [k0, k1) of a kvol-27 map and a
+       layer with one offset per accumulation group (c1 + c2 >= 176), so a conv split into ascending contiguous ranges, run as
+       one launch per range, adds the same products in the same order as one launch over all 27 and gives the same bits (up to
+       the sign of an exactly zero sum).  A range launch dispatches the rows row_perm[0 .. *d_mout): for a range that is not
+       the last, lb2_row_order_range's live rows and d_live; for the last range, every row (d_mout = the map's row count).
+       Each dispatched row starts from partial_in[pass][row] when its row_mask has a bit in [0, k0) (else from -0); a launch
+       with partial_out writes its unscaled fp32 sums to partial_out[pass][row] and nothing else (no BN, residual, gate or
+       outputs), a launch without it runs the epilogue.  partial_in / partial_out: (npass, mout_cap, cout) fp32, may be the same
+       buffer.  row_mask is required.  k1 == 0: all offsets, partial_in / partial_out unused. */
+    int32_t        k0, k1;
+    const float*   partial_in;
+    float*         partial_out;
 } lb2_conv_desc;
 
 #define LB2_ALGO_AUTO  0

@@ -36,7 +36,8 @@ class ConvDesc(C.Structure):
                 ("d_mout", C.c_void_p), ("mout_cap", C.c_int32), ("row_perm", C.c_void_p), ("row_mask", C.c_void_p),
                 ("npass", C.c_int32),
                 ("io", ConvIO * 2),
-                ("tile_order128", C.c_void_p), ("tile_order256", C.c_void_p)]
+                ("tile_order128", C.c_void_p), ("tile_order256", C.c_void_p),
+                ("k0", C.c_int32), ("k1", C.c_int32), ("partial_in", C.c_void_p), ("partial_out", C.c_void_p)]
 
 
 class ScatterDesc(C.Structure):
@@ -57,7 +58,7 @@ class DpmCoef(C.Structure):
 
 EXPORTS = [
     "lb2_create", "lb2_destroy", "lb2_last_error", "lb2_version", "lb2_launch_count", "lb2_read_status",
-    "lb2_tile_order",
+    "lb2_tile_order", "lb2_row_order_range", "lb2_tile_order_range",
     "lb2_quantize", "lb2_unique_scratch_bytes", "lb2_unique_build", "lb2_voxel_mean_scratch_bytes", "lb2_voxel_mean", "lb2_kernel_map",
     "lb2_spconv_forward", "lb2_packed_weight_bytes", "lb2_pack_weights", "lb2_nn_match", "lb2_linear",
     "lb2_gate_mul", "lb2_gather_rows", "lb2_head_mlp", "lb2_kernel_map_self", "lb2_guidance_dpm_step", "lb2_farthest_point_sample",
@@ -116,6 +117,8 @@ class Lib:
         d.lb2_kernel_map_self.argtypes = [vp, vp, Grid, vp, vp, i32, i32, vp, i64, vp, vp]
         d.lb2_row_order.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, i32]
         d.lb2_tile_order.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp, vp]
+        d.lb2_row_order_range.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp]
+        d.lb2_tile_order_range.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, vp, vp]
         d.lb2_row_order_scratch_bytes.restype = C.c_size_t
         d.lb2_row_order_scratch_bytes.argtypes = [i32]
         d.lb2_spconv_forward.argtypes = [vp, vp, C.POINTER(ConvDesc), C.c_int]
@@ -249,6 +252,14 @@ class Handle:
     def tile_order(self, row_mask, row_perm, d_n, n_cap, order128, order256, scratch):
         self._check(self.dll.lb2_tile_order(self.hp, self._stream(), _ptr(row_mask), _ptr(row_perm), _ptr(d_n), int(n_cap), _ptr(order128),
                                             _ptr(order256), _ptr(scratch)), "lb2_tile_order")
+
+    def row_order_range(self, row_mask, d_n, n_cap, k0, k1, perm, d_live, scratch):
+        self._check(self.dll.lb2_row_order_range(self.hp, self._stream(), _ptr(row_mask), _ptr(d_n), int(n_cap), int(k0), int(k1), _ptr(perm),
+                                                 _ptr(d_live), _ptr(scratch)), "lb2_row_order_range")
+
+    def tile_order_range(self, row_mask, row_perm, d_n, n_cap, k0, k1, order128, scratch):
+        self._check(self.dll.lb2_tile_order_range(self.hp, self._stream(), _ptr(row_mask), _ptr(row_perm), _ptr(d_n), int(n_cap), int(k0), int(k1),
+                                                  _ptr(order128), _ptr(scratch)), "lb2_tile_order_range")
 
     # -- conv ----------------------------------------------------------------------------------------
     def spconv(self, desc: ConvDesc, algo: int = ALGO_AUTO):

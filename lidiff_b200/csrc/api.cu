@@ -26,6 +26,11 @@ extern "C" int lb2_spconv_forward(void* handle, void* stream, const lb2_conv_des
     }
     LB2_REQUIRE(h, d->c2 == 0 || d->c1 % 16 == 0, "c1 must be a multiple of 16 when in2 is given");
     cudaStream_t s = (cudaStream_t)stream;
+    if (d->k1 > 0) {                                       // offset ranges: the tensor-core variant only
+        if (algo == LB2_ALGO_FFMA || !d->weight_packed || !lb2_spconv_tc_supported(d))
+            return lb2_fail(h, LB2_ERR_UNSUP, "an offset range needs the tensor-core variant%s", "");
+        return lb2_spconv_tc_launch(h, s, d);
+    }
     if (algo == LB2_ALGO_TC || algo == LB2_ALGO_TC_TILE) {
         if (!d->weight_packed || !lb2_spconv_tc_supported(d))
             return lb2_fail(h, LB2_ERR_UNSUP, "tensor-core variant does not support this layer%s", "");

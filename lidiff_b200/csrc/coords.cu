@@ -526,6 +526,23 @@ __device__ __forceinline__ unsigned ro_key27(unsigned mask) {
     return ((__popc(extras) >= 2) ? (1u << 26) : 0u) | k26;
 }
 
+// key of the row order of an offset range [k0, k1) (lb2_row_order_range): [sub == 0 | 2 or more off-centre bits of sub | sub without the
+// centre bit, compacted to the range], sub = mask & bits [k0, k1); ro_key_bits(k0, k1) bits wide.  Over [0, 27) the low 27 bits are
+// ro_key27's key.
+__device__ __host__ __forceinline__ int ro_range_nb(int k0, int k1) { return (k1 - k0) - ((k0 <= 13 && 13 < k1) ? 1 : 0); }
+__device__ __host__ __forceinline__ unsigned ro_range_mask(int k0, int k1) { return ((1u << k1) - 1u) & ~((1u << k0) - 1u); }
+__device__ __forceinline__ unsigned ro_key_range(unsigned mask, int k0, int k1) {
+    const unsigned sub = mask & ro_range_mask(k0, k1);
+    const int nb = ro_range_nb(k0, k1);
+    unsigned local = sub >> k0;
+    if (k0 <= 13 && 13 < k1) {
+        const int c = 13 - k0;
+        local = ((local >> (c + 1)) << c) | (local & ((1u << c) - 1u));
+    }
+    const unsigned multi = __popc(sub & ~(1u << 13)) >= 2 ? 1u : 0u;
+    return ((sub == 0u ? 1u : 0u) << (nb + 1)) | (multi << nb) | local;
+}
+
 // 27-bit Morton code of a row's voxel coordinate (9 bits per axis of coord >> shift; wraps beyond 512 cells: locality hint only)
 __device__ __forceinline__ unsigned ro_part9(unsigned v) {           // 9 bits -> every third bit
     v &= 0x1ffu;
@@ -546,8 +563,9 @@ struct RsSrc {
                                  // mode 3: ro_key27(mask[vals_in[i]])   (first mask pass behind the Morton passes)
                                  // mode 4: mask[i] & 0xff               (the one pass of an 8-bit mask sort, value = i)
     const int4* coords;          // mode 2: ro_morton(coords[i])          (first Morton pass, value = i)
+                                 // mode 5: ro_key_range(mask[i], k0, k1)   (first pass of a range sort, value = i)
     const int* vals;             // values of the previous pass or NULL (value = i)
-    int mode, coord_shift;
+    int mode, coord_shift, k0, k1;
 };
 __device__ __forceinline__ unsigned rs_key(const RsSrc& s, int i) {
     switch (s.mode) {
@@ -555,6 +573,7 @@ __device__ __forceinline__ unsigned rs_key(const RsSrc& s, int i) {
         case 1: return ro_key27(s.mask[i]);
         case 2: return ro_morton(s.coords[i], s.coord_shift);
         case 4: return s.mask[i] & 0xffu;
+        case 5: return ro_key_range(s.mask[i], s.k0, s.k1);
         default: return ro_key27(s.mask[s.vals[i]]);
     }
 }
@@ -695,6 +714,50 @@ extern "C" int lb2_row_order(void* handle, void* stream, const uint32_t* row_mas
     LB2_POST_LAUNCH(h, "k_rs_hist");
     k_rs_scatter<<<nblk, 32 * RS_WARPS, 0, s>>>(src, d_n, n_cap, 0, hist, total, nullptr, perm);
     LB2_POST_LAUNCH(h, "k_rs_scatter");
+    return LB2_OK;
+}
+
+__global__ void __launch_bounds__(256) k_range_live(const unsigned* __restrict__ mask, const int* __restrict__ d_n, int n_cap, unsigned rmask,
+                                                    int* __restrict__ d_live) {
+    const int n = d_n ? min(*d_n, n_cap) : n_cap;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned live = __ballot_sync(0xffffffffu, i < n && (__ldg(mask + i) & rmask) != 0u);
+    if ((threadIdx.x & 31) == 0 && live) atomicAdd(d_live, __popc(live));
+}
+
+extern "C" int lb2_row_order_range(void* handle, void* stream, const uint32_t* row_mask, const int32_t* d_n, int32_t n_cap, int32_t k0, int32_t k1,
+                                   int32_t* perm, int32_t* d_live, void* scratch) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h && row_mask && perm && d_live && scratch && n_cap > 0, "row_order_range");
+    LB2_REQUIRE(h, 0 <= k0 && k0 < k1 && k1 <= 27, "row_order_range: offset range outside [0, 27)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int nblk = rs_blocks(n_cap);
+    int* hist = (int*)scratch;
+    int* total = hist + (size_t)RS_BINS * nblk;
+    unsigned* keys_a = (unsigned*)(total + 6 * RS_BINS);
+    unsigned* keys_b = keys_a + n_cap;
+    int* vals_a = (int*)(keys_b + n_cap);
+    const int npass = cdiv(ro_range_nb(k0, k1) + 2, RS_BITS);          // 2 .. 4 passes
+    if (cudaMemsetAsync(total, 0, (size_t)npass * RS_BINS * sizeof(int), s) != cudaSuccess ||
+        cudaMemsetAsync(d_live, 0, sizeof(int32_t), s) != cudaSuccess)
+        return lb2_fail(h, LB2_ERR_CUDA, "row_order_range memset%s", "");
+    k_range_live<<<cdiv(n_cap, 256), 256, 0, s>>>(row_mask, d_n, n_cap, ro_range_mask(k0, k1), d_live);
+    LB2_POST_LAUNCH(h, "k_range_live");
+    // LSD passes; the values alternate between vals_a and perm so that the last pass writes perm
+    for (int pass = 0; pass < npass; ++pass) {
+        const bool to_perm = ((npass - 1 - pass) & 1) == 0;
+        RsSrc src;
+        src.mask = row_mask; src.coords = nullptr; src.coord_shift = 0; src.k0 = k0; src.k1 = k1;
+        src.keys = (pass & 1) ? keys_a : keys_b;
+        src.vals = (pass == 0) ? nullptr : (to_perm ? vals_a : perm);
+        src.mode = (pass == 0) ? 5 : 0;
+        unsigned* kout = (pass == npass - 1) ? nullptr : ((pass & 1) ? keys_b : keys_a);
+        int* vout = to_perm ? perm : vals_a;
+        k_rs_hist<<<nblk, 256, 0, s>>>(src, d_n, n_cap, pass * RS_BITS, hist, total + pass * RS_BINS);
+        LB2_POST_LAUNCH(h, "k_rs_hist");
+        k_rs_scatter<<<nblk, 32 * RS_WARPS, 0, s>>>(src, d_n, n_cap, pass * RS_BITS, hist, total + pass * RS_BINS, kout, vout);
+        LB2_POST_LAUNCH(h, "k_rs_scatter");
+    }
     return LB2_OK;
 }
 
@@ -894,7 +957,7 @@ extern "C" int lb2_nn_tree_build(void* handle, void* stream, const int32_t* k_co
 //   order128[i] / order256[i] = index of the i-th most expensive tile; entries beyond the live tile count are -1.
 // ---------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_tile_masks(const unsigned* __restrict__ mask, const int* __restrict__ perm, const int* __restrict__ d_n,
-                                                    int n_cap, unsigned* __restrict__ tmask) {
+                                                    int n_cap, unsigned kmask, unsigned* __restrict__ tmask) {
     const int n = d_n ? min(*d_n, n_cap) : n_cap;
     const int nt = (n + 127) >> 7;
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -906,7 +969,7 @@ __global__ void __launch_bounds__(256) k_tile_masks(const unsigned* __restrict__
         if (slot < n) m |= __ldg(mask + (perm ? __ldg(perm + slot) : slot));
     }
     m = __reduce_or_sync(0xffffffffu, m);
-    if (lane == 0) tmask[warp] = m;
+    if (lane == 0) tmask[warp] = m & kmask;
 }
 
 __global__ void __launch_bounds__(1024) k_tile_sort(const unsigned* __restrict__ tmask, const int* __restrict__ d_n, int n_cap,
@@ -919,7 +982,7 @@ __global__ void __launch_bounds__(1024) k_tile_sort(const unsigned* __restrict__
     __syncthreads();
     // histogram of costs (0..32), descending order: bin b holds cost 32 - b
     for (int t = threadIdx.x; t < nt128; t += blockDim.x) atomicAdd(&bins[0][32 - __popc(tmask[t])], 1);
-    for (int u = threadIdx.x; u < nt256; u += blockDim.x) {
+    for (int u = threadIdx.x; order256 && u < nt256; u += blockDim.x) {
         const unsigned m = tmask[2 * u] | ((2 * u + 1 < nt128) ? tmask[2 * u + 1] : 0u);
         atomicAdd(&bins[1][32 - __popc(m)], 1);
     }
@@ -930,12 +993,12 @@ __global__ void __launch_bounds__(1024) k_tile_sort(const unsigned* __restrict__
     }
     __syncthreads();
     for (int t = threadIdx.x; t < nt128; t += blockDim.x) order128[atomicAdd(&bins[0][32 - __popc(tmask[t])], 1)] = t;
-    for (int u = threadIdx.x; u < nt256; u += blockDim.x) {
+    for (int u = threadIdx.x; order256 && u < nt256; u += blockDim.x) {
         const unsigned m = tmask[2 * u] | ((2 * u + 1 < nt128) ? tmask[2 * u + 1] : 0u);
         order256[atomicAdd(&bins[1][32 - __popc(m)], 1)] = u;
     }
     for (int t = nt128 + threadIdx.x; t < cap128; t += blockDim.x) order128[t] = -1;
-    for (int u = nt256 + threadIdx.x; u < cap256; u += blockDim.x) order256[u] = -1;
+    for (int u = nt256 + threadIdx.x; order256 && u < cap256; u += blockDim.x) order256[u] = -1;
 }
 
 extern "C" int lb2_tile_order(void* handle, void* stream, const uint32_t* row_mask, const int32_t* row_perm, const int32_t* d_n, int32_t n_cap,
@@ -944,9 +1007,23 @@ extern "C" int lb2_tile_order(void* handle, void* stream, const uint32_t* row_ma
     LB2_REQUIRE(h, h && row_mask && order128 && order256 && scratch && n_cap > 0, "tile_order");
     cudaStream_t s = (cudaStream_t)stream;
     const int cap128 = cdiv(n_cap, 128);
-    k_tile_masks<<<cdiv(cap128, 8), 256, 0, s>>>(row_mask, row_perm, d_n, n_cap, (unsigned*)scratch);
+    k_tile_masks<<<cdiv(cap128, 8), 256, 0, s>>>(row_mask, row_perm, d_n, n_cap, 0xffffffffu, (unsigned*)scratch);
     LB2_POST_LAUNCH(h, "k_tile_masks");
     k_tile_sort<<<1, 1024, 0, s>>>((const unsigned*)scratch, d_n, n_cap, order128, order256);
+    LB2_POST_LAUNCH(h, "k_tile_sort");
+    return LB2_OK;
+}
+
+extern "C" int lb2_tile_order_range(void* handle, void* stream, const uint32_t* row_mask, const int32_t* row_perm, const int32_t* d_n, int32_t n_cap,
+                                    int32_t k0, int32_t k1, int32_t* order128, void* scratch) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h && row_mask && order128 && scratch && n_cap > 0, "tile_order_range");
+    LB2_REQUIRE(h, 0 <= k0 && k0 < k1 && k1 <= 27, "tile_order_range: offset range outside [0, 27)");
+    cudaStream_t s = (cudaStream_t)stream;
+    const int cap128 = cdiv(n_cap, 128);
+    k_tile_masks<<<cdiv(cap128, 8), 256, 0, s>>>(row_mask, row_perm, d_n, n_cap, ro_range_mask(k0, k1), (unsigned*)scratch);
+    LB2_POST_LAUNCH(h, "k_tile_masks");
+    k_tile_sort<<<1, 1024, 0, s>>>((const unsigned*)scratch, d_n, n_cap, order128, nullptr);
     LB2_POST_LAUNCH(h, "k_tile_sort");
     return LB2_OK;
 }

@@ -27,6 +27,10 @@
 //                The totals go through the epilogue slot to a coalesced epilogue:
 //                BN affine + residual + ReLU + gate -> global.
 // Kernel offsets where none of the tile's 128 rows has a neighbour are skipped by every role.
+// OFFSET RANGES: a launch may run only the offsets [k0, k1) of a layer whose groups hold one offset each (range_mask = those bits).
+// A row then starts its totals from partial_in when its mask has a bit below k0 (prior_mask), and a launch that is not the layer's
+// last writes its unscaled totals to partial_out instead of running the epilogue.  The adds are those of one launch over all offsets,
+// in the same order.
 //
 // Stands behind ME.MinkowskiConvolution(+Transpose) forward (lidiff/models/minkunet.py of the reference).
 #include "common.cuh"
@@ -60,6 +64,9 @@ struct Params {
     int stages, nchunks, group;                         // group: kernel offsets per accumulation group
     int npass, nsplit;
     lb2_conv_io io[2];
+    uint32_t range_mask, prior_mask;                    // offsets of this launch / below it (~0u / 0 without a range)
+    const float* partial_in;                            // (npass, mout_cap, cout) totals of the offsets below the range, or NULL
+    float* partial_out;                                 // same layout: this launch's totals (no epilogue), or NULL
 };
 
 // Registers per thread after the producer warpgroup hands its surplus to the consumers.  The CTA is launched with 168 per thread
@@ -76,6 +83,7 @@ struct TileInfo {
     int idx[MAX_KVOL * BM];      // neighbour row of (kernel offset k, tile row r) at [k * BM + r], -1 = none
     int row[BM];                 // output row of each tile row, -1 beyond the live rows
     uint32_t mask[4];            // per producer warp: OR of its rows' offset masks
+    uint32_t prior[4];           // bit r & 31 of word r >> 5: tile row r starts from partial_in
     int item;                    // work item, -1 = this CTA has no more
     int pad[3];
 };
@@ -132,18 +140,22 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
         };
         // index loads of tile row threadIdx.x: its output row and the neighbour row of every kernel offset (-1 = none).  The row's
         // neighbour mask names the offsets that have an entry: only those index loads are issued, all at once (the sparse levels' rows
-        // have a few of 27, and the loads hit random rows of the map).  Without a mask every offset is loaded.
+        // have a few of 27, and the loads hit random rows of the map).  Without a mask every offset is loaded.  A row whose mask has an
+        // offset below the launch's range (it starts from partial_in) gets bit 30 of `row` set (rows < 2^22), so that no register
+        // lives across the loop for it.
         auto load_row = [&](int tile) {
             const int slot = tile * BM + threadIdx.x;
             return (tile >= 0 && slot < M) ? (p.row_perm ? __ldg(p.row_perm + slot) : slot) : -1;
         };
-        auto load_indices = [&](int row, int (&v)[MAX_KVOL]) {
-            const uint32_t want = row < 0 ? 0u : (p.row_mask ? __ldg(p.row_mask + row) : ~0u);
+        auto load_indices = [&](int& row, int (&v)[MAX_KVOL]) {
+            const uint32_t m = row < 0 ? 0u : (p.row_mask ? __ldg(p.row_mask + row) : ~0u);
+            const uint32_t want = m & p.range_mask;
 #pragma unroll
             for (int k = 0; k < MAX_KVOL; ++k) {
                 v[k] = -1;
-                if (k < p.kvol && ((want >> k) & 1u)) v[k] = p.nbr ? __ldg(p.nbr + (long long)k * p.nbr_stride + row) : row;
+                if (k < p.kvol && (want >> k) & 1u) v[k] = p.nbr ? __ldg(p.nbr + (long long)k * p.nbr_stride + row) : row;
             }
+            if (m & p.prior_mask) row |= 1 << 30;         // after the index loads, which address with the plain row
         };
         int x = blockIdx.x, tile = tile_of(x), row = load_row(tile), v[MAX_KVOL];
         load_indices(row, v);
@@ -157,7 +169,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
             }
             // ---- the tile's index table + mask of non-empty kernel offsets: one thread per tile row ----
             {
-                ti.row[threadIdx.x] = row;
+                ti.row[threadIdx.x] = row < 0 ? row : row & ~(1 << 30);
                 uint32_t have = 0;
 #pragma unroll
                 for (int k = 0; k < MAX_KVOL; ++k) {
@@ -167,7 +179,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
                     }
                 }
                 const uint32_t wmask = __reduce_or_sync(0xffffffffu, have);
-                if (lane == 0) ti.mask[warp] = wmask;
+                const uint32_t wprior = __ballot_sync(0xffffffffu, row >= 0 && (row >> 30));
+                if (lane == 0) { ti.mask[warp] = wmask; ti.prior[warp] = wprior; }
                 if (threadIdx.x == 0) ti.item = x;
             }
             mbar_arrive(info_full(j & 1));
@@ -242,10 +255,30 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
             const int x = ti.item;
             if (x < 0) break;
             const int n_off = __popc(ti.mask[0] | ti.mask[1] | ti.mask[2] | ti.mask[3]);
-            // tot starts at -0: -0 + x == x for every x (+0 and -0 included), so the first fold is an exact copy without a select
+            // tot starts at -0: -0 + x == x for every x (+0 and -0 included), so the first fold is an exact copy without a select.
+            // A row of a range launch with offsets below the range starts from the totals they left in partial_in.
             float acc[NC / 2], tot[NC / 2];
+            if (p.partial_in) {
+                const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // this thread's fragment rows: r0, r0 + 8
+                const float* src[2];
 #pragma unroll
-            for (int i = 0; i < NC / 2; ++i) tot[i] = -0.f;
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int rr = r0 + 8 * hh;
+                    const bool pr = (ti.prior[rr >> 5] >> (rr & 31)) & 1u;
+                    src[hh] = pr ? p.partial_in + ((long long)((x / p.nsplit) % p.npass) * p.mout_cap + ti.row[rr]) * p.cout + (x % p.nsplit) * NC
+                                 : nullptr;
+                }
+#pragma unroll
+                for (int i = 0; i < NC / 2; i += 2) {
+                    const float* q = src[(i >> 1) & 1];
+                    const float2 t = q ? __ldcg(reinterpret_cast<const float2*>(q + 8 * (i >> 2) + 2 * (lane & 3))) : make_float2(-0.f, -0.f);
+                    tot[i] = t.x;
+                    tot[i + 1] = t.y;
+                }
+            } else {
+#pragma unroll
+                for (int i = 0; i < NC / 2; ++i) tot[i] = -0.f;
+            }
             // one flat loop over the tile's stages (offset-major, chunk-minor), the stage sequence the producers publish
             const int n_it = n_off * p.nchunks;
             int c = 0, in_group = 0, off_idx = 0, prev_s = -1;
@@ -288,11 +321,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
             float* stage_c = reinterpret_cast<float*>(gen + (size_t)se * stage_bytes);
             {
                 const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+                const float sc = p.partial_out ? 1.f : out_scale;         // partial totals stay unscaled (x * 1 == x)
 #pragma unroll
                 for (int i = 0; i < NC / 2; i += 2) {
                     const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3);
                     *reinterpret_cast<float2*>(stage_c + row * NC + (((col >> 2) ^ (row & 7)) << 2) + (col & 3)) =
-                        make_float2(tot[i] * out_scale, tot[i + 1] * out_scale);
+                        make_float2(tot[i] * sc, tot[i + 1] * sc);
                 }
             }
             asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -311,7 +345,18 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
             const bool has_res = io.residual || io.residual_h;
             const bool gated = io.out_gated || io.out_gated_h;
             const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            for (int e0 = 0; e0 < PER_LANE; e0 += EPI_BATCH) {
+            if (p.partial_out) {        // a range launch that is not the layer's last: the totals only, coalesced as below
+                float* dst = p.partial_out + (long long)((x / p.nsplit) % p.npass) * p.mout_cap * p.cout;
+                for (int e = lane; e < PER_LANE * 32; e += 32) {
+                    const int rr = cw + NUM_CONSUMER_WARPS * (e / nv);
+                    const int lcol = (e % nv) * 4;
+                    const int orow = ti.row[rr];
+                    if (orow >= 0)
+                        __stcg(reinterpret_cast<float4*>(dst + (long long)orow * p.cout + n0 + lcol),
+                               *reinterpret_cast<const float4*>(stage_c + rr * NC + (((lcol >> 2) ^ (rr & 7)) << 2)));
+                }
+            }
+            for (int e0 = 0; !p.partial_out && e0 < PER_LANE; e0 += EPI_BATCH) {
                 int orow[EPI_BATCH], col[EPI_BATCH];
                 long long gi[EPI_BATCH];
                 float4 a4[EPI_BATCH], pre4[EPI_BATCH], s4[EPI_BATCH], h4[EPI_BATCH], res4[EPI_BATCH], g4[EPI_BATCH];
@@ -489,6 +534,18 @@ int lb2_spconv_tc_launch(Lb2Handle* h, cudaStream_t s, const lb2_conv_desc* d) {
     const int steps_per_offset = 3 * ((d->c1 + d->c2 + 15) / 16);
     p.group = std::max(1, tc::STEP_BUDGET / steps_per_offset);
     p.io[0] = d->io[0]; p.io[1] = d->io[d->npass > 1 ? 1 : 0];
+    p.range_mask = ~0u; p.prior_mask = 0u; p.partial_in = nullptr; p.partial_out = nullptr;
+    if (d->k1 > 0) {
+        // the same bits as one launch need one offset per accumulation group: then every offset is one RN add to the total
+        if (d->kvol != 27 || !d->nbr || !d->row_mask || d->k0 < 0 || d->k0 >= d->k1 || d->k1 > 27 || p.group != 1 ||
+            (d->k0 > 0) != (d->partial_in != nullptr) || (d->k1 < 27) != (d->partial_out != nullptr))
+            return lb2_fail(h, LB2_ERR_ARG, "offset range: needs kvol 27, a map with row masks, c1 + c2 >= 176, 0 <= k0 < k1 <= 27, "
+                                            "partial_in iff k0 > 0 and partial_out iff k1 < 27%s", "");
+        p.range_mask = ((1u << d->k1) - 1u) & ~((1u << d->k0) - 1u);
+        p.prior_mask = (1u << d->k0) - 1u;
+        p.partial_in = d->partial_in;
+        p.partial_out = d->partial_out;
+    }
     switch (nc) {
         case 32: return tc::launch<32>(h, s, p, stages);
         case 64: return tc::launch<64>(h, s, p, stages);

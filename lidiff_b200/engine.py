@@ -21,6 +21,7 @@ from __future__ import annotations
 
 import math
 import os
+import re
 from collections import ChainMap
 
 import numpy as np
@@ -33,6 +34,44 @@ from .scheduler import DPMSolverMultistepScheduler
 GATE_NAMES = ("stage1", "stage2", "stage3", "stage4", "up1", "up2", "up3", "up4")
 GATE_LEVEL = (0, 1, 2, 3, 4, 3, 2, 1)
 BN_EPS = 1e-5
+
+# Offset split of the 3^3 convolutions with one kernel offset per accumulation group (c1 + c2 >= 176: stage 4, up1 and up2's first
+# conv, in both U-Nets): G launches over contiguous offset ranges, each with the row and tile order of its own range, carrying the
+# fp32 totals from one range to the next.  Same bits as one launch (lb2_conv_desc.k0 / k1); fewer MMAs on absent offsets, because a
+# 128-row tile of rows sorted by a 9- or 13-bit sub-mask is far more homogeneous than one sorted by the 27-bit mask.
+OFFSET_RANGES = {2: ((0, 14), (14, 27)), 3: ((0, 9), (9, 18), (18, 27))}
+# G per residual-block group, from scripts/bench_offset_split.py on the H100 (DESIGN.md §3); LB2_OFFSET_SPLIT overrides it for A/B
+# runs: "1", "2" or "3" for every such layer, or "stage4=3,up1=2,up2=1".
+OFFSET_SPLIT_DEFAULT = {"stage4": 3, "up1": 3, "up2": 3}
+
+
+def offset_split_table(env=None):
+    env = os.environ.get("LB2_OFFSET_SPLIT", "") if env is None else env
+    table = dict(OFFSET_SPLIT_DEFAULT)
+    env = env.strip()
+    if env.isdigit():
+        return {k: int(env) for k in table}
+    for item in filter(None, env.split(",")):
+        k, _, v = item.partition("=")
+        table[k.strip()] = int(v)
+    for k, g in table.items():
+        if g != 1 and g not in OFFSET_RANGES:
+            raise ValueError(f"LB2_OFFSET_SPLIT: {k}={g} (G must be 1, 2 or 3)")
+    return table
+
+
+def split_level(name: str):
+    """(block group, level) of a 3^3 residual-block conv of the U-Nets (stage<n>.1/2 at level n, up<n>.1.* at level 4 - n), else None"""
+    m = re.match(r"(stage(\d))\.[12]\.net\.[03]$", name) or re.match(r"(up(\d))\.1\.[01]\.net\.[03]$", name)
+    if m is None:
+        return None
+    n = int(m.group(2))
+    return m.group(1), (n if name.startswith("stage") else 4 - n)
+
+
+def one_offset_per_group(cin: int) -> bool:
+    """the tensor-core conv's accumulation groups hold one offset each (lb2_spconv_tc_launch: 64 // (3 ceil(cin / 16)) <= 1)"""
+    return 64 // (3 * ((cin + 15) // 16)) <= 1
 
 
 class ConvLayer:
@@ -149,6 +188,9 @@ class Geometry:
         self.pairs_of = {}
         self.pl_scratch = torch.zeros(64, **i32)
         want = [use_pairs and l in self.pair_level_set for l in range(self.pair_levels)]     # 208 B/row per level: only where asked for
+        # offset split: level -> the G whose range orders are built, (map, G) -> [(k0, k1, perm, live rows, tile order)]
+        self.split_groups = {}
+        self.range_of = {}
         self.pair_in = [torch.zeros(26 * n_cap, **i32) if w else None for w in want]
         self.pair_out = [torch.zeros(26 * n_cap, **i32) if w else None for w in want]
         self.koff = [torch.zeros(28, **i32) for _ in range(self.pair_levels)]
@@ -162,6 +204,7 @@ class Geometry:
         stream, all others on `late_stream` (own scratch buffers), `late_done` recorded behind them: the caller waits for it in front
         of the first layer of stage 2, so ~0.6 ms of map construction hides behind the stem and stage-1 convolutions."""
         h, N = self.h, self.n_cap
+        i32 = dict(dtype=torch.int32, device=coords_f.device)
         h.unique_build(coords_f, None, None, n_points, 0, self.grid[0], self.C[0], self.inv[0], self.d_n[0], self.scratch)
         for l in range(1, self.levels):
             h.unique_build(None, self.C[l - 1], self.d_n[l - 1], N, 1 << l, self.grid[l], self.C[l], self.inv[l], self.d_n[l], self.scratch)
@@ -188,6 +231,14 @@ class Geometry:
                     to = self.tile_order_of[nbr.data_ptr()] = (torch.zeros((N + 127) // 128, dtype=torch.int32, device=nbr.device),
                                                                torch.zeros((N + 255) // 256, dtype=torch.int32, device=nbr.device))
                 h.tile_order(mask, perm, self.d_n[l_out], N, to[0], to[1], to_scratch)
+            for G in (sorted(self.split_groups.get(l_out, ())) if ks == 3 else ()):
+                ent = self.range_of.get((nbr.data_ptr(), G))
+                if ent is None:
+                    ent = self.range_of[(nbr.data_ptr(), G)] = [
+                        (k0, k1, torch.zeros(N, **i32), torch.zeros(1, **i32), torch.zeros((N + 127) // 128, **i32)) for k0, k1 in OFFSET_RANGES[G]]
+                for k0, k1, perm_r, live_r, to_r in ent:
+                    h.row_order_range(mask, self.d_n[l_out], N, k0, k1, perm_r, live_r, ro_scratch)
+                    h.tile_order_range(mask, perm_r, self.d_n[l_out] if k1 == 27 else live_r, N, k0, k1, to_r, to_scratch)
             self.map_id[nbr.data_ptr()] = slot
             self.perm_of[nbr.data_ptr()] = perm
 
@@ -302,6 +353,19 @@ class DenoiseEngine:
         self._perm_lookup = {}
         self._tile_order_lookup = {}
         self.geom = Geometry(h, self.cap, with_up=True)
+        # offset split: G per conv layer (1 = one launch); range orders only on the step geometry and a backend that builds them
+        self.split_of = {}
+        if hasattr(h, "row_order_range") and conv_algo != _lib.ALGO_FFMA:
+            table = offset_split_table()
+            for net in (self.diff, self.refine or {}):
+                for name, lay in net.items():
+                    sl = split_level(name)
+                    if sl is None or lay.kvol != 27 or lay.Wp is None or not one_offset_per_group(lay.cin):
+                        continue
+                    G = table.get(sl[0], 1)
+                    if G > 1:
+                        self.split_of[id(lay)] = G
+                        self.geom.split_groups.setdefault(sl[1], set()).add(G)
         self._perm_lookup = self.geom.perm_of
         self._mask_lookup = self.geom.mask_of
         self._tile_order_lookup = self.geom.tile_order_of
@@ -488,18 +552,36 @@ class DenoiseEngine:
             self.layer_log.append(dict(name=lay.name, scatter=sd is not None, map=map_ptr, d_m=d_m.data_ptr() if d_m is not None else None,
                                        cin=lay.cin, cout=lay.cout, kvol=lay.kvol, npass=npass,
                                        tc=bool(lay.Wp is not None and self.conv_algo != _lib.ALGO_FFMA)))
+        ranges = None
+        if sd is None and perm is not None and id(lay) in self.split_of:
+            ranges = self.geom.range_of.get((nbr.data_ptr(), self.split_of[id(lay)]))
         if self.conv_events is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             if sd is not None:
                 self.h.spconv_scatter(sd)
-            self.h.spconv(d, self.conv_algo)
+            self._spconv(d, ranges, d_m, cap)
             e1.record()
             self.conv_events.append((e0, e1, self._conv_counter))
             self._conv_counter += 1
         else:
             if sd is not None:
                 self.h.spconv_scatter(sd)
+            self._spconv(d, ranges, d_m, cap)
+
+    def _spconv(self, d, ranges, d_m, cap):
+        """one launch, or one per offset range (each with its range's row order, tile order and live rows) carrying the fp32 totals
+        through one (2, cap, 256) buffer in place"""
+        if ranges is None:
+            self.h.spconv(d, self.conv_algo)
+            return
+        part = self.buf("offset_split.partial", (2, cap, 256)).data_ptr()
+        for k0, k1, perm_r, live_r, to_r in ranges:
+            d.row_perm, d.tile_order128, d.tile_order256 = perm_r.data_ptr(), to_r.data_ptr(), None
+            d.d_mout = (d_m if k1 == 27 else live_r).data_ptr()
+            d.k0, d.k1 = k0, k1
+            d.partial_in = part if k0 > 0 else None
+            d.partial_out = part if k1 < 27 else None
             self.h.spconv(d, self.conv_algo)
 
     def _res(self, L, p, geom, lvl, in1: Act, in2: Act, npass, tag, gate=None, want_plain=True, lean=False, out_f32=False):
@@ -863,8 +945,9 @@ class DenoiseEngine:
 
 
 # device bytes per point row of a whole completion with the engine: the peak of scripts/bench_batch.py on an H100 80GB HBM3 is
-# 117.1-117.8 KB at 180 000 points per scan (B = 1, 2, 3), plus a margin for the allocator's rounding
-ENGINE_BYTES_PER_ROW = 120_000
+# 117.1-117.8 KB at 180 000 points per scan (B = 1, 2, 3) before the offset split's (2, rows, 256) fp32 partial-total buffer
+# (2 KB per row) was added; that buffer plus a margin for the allocator's rounding
+ENGINE_BYTES_PER_ROW = 122_000
 MAX_BATCH = 1 << 10                  # coordinate keys carry 10 batch bits (csrc/common.cuh)
 
 
