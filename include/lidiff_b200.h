@@ -448,6 +448,48 @@ size_t lb2_map_scan_scratch_bytes(int32_t n_cap);
 int lb2_map_scan(void* h, void* stream, const float* points, const uint32_t* labels, int32_t n, lb2_pose pose, float voxel_size,
                  int32_t div_mode, lb2_grid table, float* map, int32_t map_n, int32_t map_cap, int32_t* d_out, void* scratch);
 
+/* ---- training / test samples — lidiff/datasets/dataloader/SemanticKITTITemporal.py:82-105 and lidiff/utils/collations.py:44-51
+ * (TemporalKITTISet.__getitem__ before the farthest point sampling).  Both calls are order-preserving compactions: the kept rows
+ * are written as fp64 (x, y, z) rows in input order, *d_count (device int32) = their number.  Inputs of up to 2^31 - 1 rows. */
+
+/* lb2_select_points: row i of `points` (n rows of `stride` = 3 or 4 values, fp32 or fp64 (fp64 != 0); only x, y, z are read) is kept
+ * when every test below holds, in this order (each later test sees the row as the earlier steps left it):
+ *   finite   x, y and z are finite (numpy's comparisons with NaN are false)
+ *   labels   (uint32[n] or NULL)  1 < (l & 0xFFFF) < 252                                           (:86-91)
+ *   range    r_min < d < r_max, d = |p - center| in the input frame:
+ *              LB2_RANGE_FP32   fp32: sqrt_rn((dx*dx + dy*dy) + dz*dz), dx = fp32(x) - fp32(center.x), bounds rounded to fp32
+ *                               (the scan: a float32 array and numpy's float32 sum, :92-93)
+ *              LB2_RANGE_FP64   the same in fp64 (the map crop about the pose translation, :100-102)
+ *   transform (has_transform)  p'_k = ((m[4k] x + m[4k+1] y) + m[4k+2] z) + m[4k+3] in fp64 (the map into the scan frame, :103-104)
+ *   height   (has_z_min)  p'.z > z_min in fp64                                                          (:94, :105)
+ * Every operation is rounded on its own (no FMA contraction), so each decision is the one numpy takes on the same values.
+ * scratch >= lb2_select_points_scratch_bytes(n). */
+#define LB2_RANGE_NONE 0
+#define LB2_RANGE_FP32 1
+#define LB2_RANGE_FP64 2
+typedef struct {
+    int32_t range_mode;
+    double  center[3];
+    double  r_min, r_max;
+    int32_t has_transform;
+    double  transform[12];      /* rows 0..2 of a 4x4, row-major */
+    int32_t has_z_min;
+    double  z_min;
+} lb2_select_desc;
+size_t lb2_select_points_scratch_bytes(int64_t n);
+int lb2_select_points(void* h, void* stream, const void* points, int32_t fp64, int64_t n, int32_t stride, const uint32_t* labels,
+                      const lb2_select_desc* desc, double* out, int32_t* d_count, void* scratch);
+
+/* lb2_viewpoint_filter: o3d VoxelGrid.create_from_point_cloud(part, voxel_size).check_if_included(full) with the semantics of the
+ * open3d shim (lidiff_b200/shims/open3d/geometry.py): origin = per-axis minimum of `part` - voxel_size / 2, cell of p =
+ * floor((p - origin) / voxel_size) in fp64; row i of `full` (fp64 (n_full, 3)) is kept iff its cell holds a row of `part` (fp64
+ * (n_part, 3), finite).  Cell indices are keyed in [0, 2^21) per axis; a `full` row outside that range is not included, a `part` row
+ * outside it sets status bit 0 (the result is then incomplete).  d_out (device int32[2]): [0] = kept rows, [1] = status.
+ * An empty `part` includes nothing.  scratch >= lb2_viewpoint_filter_scratch_bytes(n_part, n_full). */
+size_t lb2_viewpoint_filter_scratch_bytes(int32_t n_part, int64_t n_full);
+int lb2_viewpoint_filter(void* h, void* stream, const double* part, int32_t n_part, const double* full, int64_t n_full,
+                         double voxel_size, double* out, int32_t* d_out, void* scratch);
+
 #ifdef __cplusplus
 }
 #endif

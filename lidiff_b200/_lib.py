@@ -70,11 +70,19 @@ EXPORTS = [
     "lb2_occupancy_bev", "lb2_jsd_scratch_bytes", "lb2_jsd", "lb2_dist_stats_scratch_bytes", "lb2_dist_stats",
     "lb2_map_rehash", "lb2_map_scan_scratch_bytes", "lb2_map_scan",
     "lb2_pc_knn", "lb2_pc_normals", "lb2_fps_batched_capacity", "lb2_farthest_point_sample_batched",
+    "lb2_select_points_scratch_bytes", "lb2_select_points", "lb2_viewpoint_filter_scratch_bytes", "lb2_viewpoint_filter",
 ]
+
+RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
 
 
 class Pose(C.Structure):
     _fields_ = [("m", C.c_float * 12)]
+
+
+class SelectDesc(C.Structure):
+    _fields_ = [("range_mode", C.c_int32), ("center", C.c_double * 3), ("r_min", C.c_double), ("r_max", C.c_double),
+                ("has_transform", C.c_int32), ("transform", C.c_double * 12), ("has_z_min", C.c_int32), ("z_min", C.c_double)]
 
 
 def _ptr(t):
@@ -163,6 +171,12 @@ class Lib:
         d.lb2_map_scan_scratch_bytes.argtypes = [i32]
         d.lb2_map_scan_scratch_bytes.restype = C.c_size_t
         d.lb2_map_scan.argtypes = [vp, vp, vp, vp, i32, Pose, f32, i32, Grid, vp, i32, i32, vp, vp]
+        d.lb2_select_points_scratch_bytes.argtypes = [i64]
+        d.lb2_select_points_scratch_bytes.restype = C.c_size_t
+        d.lb2_select_points.argtypes = [vp, vp, vp, i32, i64, i32, vp, C.POINTER(SelectDesc), vp, vp, vp]
+        d.lb2_viewpoint_filter_scratch_bytes.argtypes = [i32, i64]
+        d.lb2_viewpoint_filter_scratch_bytes.restype = C.c_size_t
+        d.lb2_viewpoint_filter.argtypes = [vp, vp, vp, i32, vp, i64, C.c_double, vp, vp, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -422,6 +436,26 @@ class Handle:
         self._check(self.dll.lb2_map_scan(self.hp, self._stream(), _ptr(points), _ptr(labels), int(points.shape[0]), pose, float(voxel_size),
                                           int(div_mode), self._grid(table), _ptr(map_buf), int(map_n), int(map_buf.shape[0]), _ptr(out),
                                           _ptr(scratch)), "lb2_map_scan")
+
+    # -- training / test samples (lidiff_b200.datasets) ---------------------------------------------------------------------------
+    def select_points_scratch(self, n: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_select_points_scratch_bytes(int(n)))
+
+    def select_points(self, points, labels, desc: SelectDesc, out, d_count, scratch):
+        """order-preserving filter + transform of the (n, 3 | 4) fp32 / fp64 rows `points` (uint32 / int32 `labels` or None) into the
+        fp64 (>= n, 3) `out`; d_count[0] = rows kept"""
+        n, stride = points.shape
+        self._check(self.dll.lb2_select_points(self.hp, self._stream(), _ptr(points), int(points.dtype == torch.float64), int(n),
+                                               int(stride), _ptr(labels), C.byref(desc), _ptr(out), _ptr(d_count), _ptr(scratch)),
+                    "lb2_select_points")
+
+    def viewpoint_filter_scratch(self, n_part: int, n_full: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_viewpoint_filter_scratch_bytes(int(n_part), int(n_full)))
+
+    def viewpoint_filter(self, part, full, voxel_size, out, d_out, scratch):
+        """rows of the fp64 (n, 3) `full` whose voxel_size cell holds a row of `part` -> `out` in order; d_out = [rows, status]"""
+        self._check(self.dll.lb2_viewpoint_filter(self.hp, self._stream(), _ptr(part), int(part.shape[0]), _ptr(full), int(full.shape[0]),
+                                                  float(voxel_size), _ptr(out), _ptr(d_out), _ptr(scratch)), "lb2_viewpoint_filter")
 
 
 _LIB = None
