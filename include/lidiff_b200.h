@@ -490,6 +490,45 @@ size_t lb2_viewpoint_filter_scratch_bytes(int32_t n_part, int64_t n_full);
 int lb2_viewpoint_filter(void* h, void* stream, const double* part, int32_t n_part, const double* full, int64_t n_full,
                          double voxel_size, double* out, int32_t* d_out, void* scratch);
 
+/* ---- refinement samples — lidiff/utils/pcd_preprocess.py:78-129 (aggregate_pcds) and
+ * lidiff/datasets/dataloader/SemanticKITTITemporalAggr.py:69-99 (TemporalKITTISet.__getitem__).  Order-preserving compactions like
+ * the two calls above: kept rows are written as fp64 (x, y, z) rows in input order.  Inputs of up to 2^31 - 1 rows, addressed with
+ * 64-bit indices; every operation is rounded on its own (no FMA contraction), in the order given. */
+
+/* lb2_aggregate_window: the scans of one window, concatenated: `points` (n, 4) fp32 rows x, y, z, remission and `labels` uint32[n].
+ * segments[nseg] (device) = the first row of every scan, ascending (segments[0].start = 0; empty scans share a start) and rows 0..2
+ * of its fp64 scan-to-world pose; undo (host, 12 fp64) = rows 0..2 of inv(pose of the window's frame).  Row i is kept when
+ *   labels   (l & 0xFFFF) < 252                    (classes 0 and 1 are kept)
+ *   range    sqrt_rn((x*x + y*y) + z*z) > 3.5 in fp32 over x, y, z       (NaN fails, +-inf passes)
+ * and written as undo(pose(p)), each p'_k = ((m[4k] x + m[4k+1] y) + m[4k+2] z) + m[4k+3] in fp64 (numpy's apply_transform).
+ * d_out (device int32[2]): [0] = kept rows, [1] = kept rows of [0, split) (the split between pcd_full and pcd_part when the frame
+ * scan is uploaded last and starts at `split`).  scratch >= lb2_aggregate_window_scratch_bytes(n). */
+typedef struct {
+    int64_t start;
+    double  m[12];
+} lb2_segment;
+size_t lb2_aggregate_window_scratch_bytes(int64_t n);
+int lb2_aggregate_window(void* h, void* stream, const float* points, const uint32_t* labels, int64_t n, const lb2_segment* segments,
+                         int32_t nseg, const double* undo, int64_t split, double* out, int32_t* d_out, void* scratch);
+
+/* lb2_jitter_filter: jitter_point_cloud (pcd_transforms.py:35-40) and the 50 m test of the noisy rows.  points, randn fp64 (n, 3);
+ * randn is numpy's standard normal draw.  w = clip(sigma * r, -clip, clip) + p per coordinate (clip: fmin(fmax(v, -clip), clip)),
+ * kept where sqrt_rn((x*x + y*y) + z*z) < max_range in fp64.  *d_count (device int32) = kept rows.
+ * scratch >= lb2_jitter_filter_scratch_bytes(n). */
+size_t lb2_jitter_filter_scratch_bytes(int64_t n);
+int lb2_jitter_filter(void* h, void* stream, const double* points, const double* randn, int64_t n, double sigma, double clip,
+                      double max_range, double* out, int32_t* d_count, void* scratch);
+
+/* lb2_voxel_first_f64: ME.utils.sparse_quantize(p / voxel_size, return_index=True) on fp64 (n, 3) rows, then the max_range test:
+ * the voxel of a row is floor(p / voxel_size) per axis (the true fp64 quotient), packed as the map keys above (+-2^20 voxels per
+ * axis); the lowest row index of every voxel wins, and a winner is kept where sqrt_rn((x*x + y*y) + z*z) < max_range in fp64.
+ * Rows with a NaN / inf coordinate are never kept.  One-shot table of the next power of two >= 2n slots.  d_out (device int32[2]):
+ * [0] = kept rows, [1] = status, bit0 = a finite row's voxel index is outside the key range (the result is then incomplete).
+ * scratch >= lb2_voxel_first_f64_scratch_bytes(n). */
+size_t lb2_voxel_first_f64_scratch_bytes(int64_t n);
+int lb2_voxel_first_f64(void* h, void* stream, const double* points, int64_t n, double voxel_size, double max_range, double* out,
+                        int32_t* d_out, void* scratch);
+
 #ifdef __cplusplus
 }
 #endif

@@ -71,6 +71,8 @@ EXPORTS = [
     "lb2_map_rehash", "lb2_map_scan_scratch_bytes", "lb2_map_scan",
     "lb2_pc_knn", "lb2_pc_normals", "lb2_fps_batched_capacity", "lb2_farthest_point_sample_batched",
     "lb2_select_points_scratch_bytes", "lb2_select_points", "lb2_viewpoint_filter_scratch_bytes", "lb2_viewpoint_filter",
+    "lb2_aggregate_window_scratch_bytes", "lb2_aggregate_window", "lb2_jitter_filter_scratch_bytes", "lb2_jitter_filter",
+    "lb2_voxel_first_f64_scratch_bytes", "lb2_voxel_first_f64",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -78,6 +80,10 @@ RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
 
 class Pose(C.Structure):
     _fields_ = [("m", C.c_float * 12)]
+
+
+class Segment(C.Structure):
+    _fields_ = [("start", C.c_int64), ("m", C.c_double * 12)]
 
 
 class SelectDesc(C.Structure):
@@ -177,6 +183,13 @@ class Lib:
         d.lb2_viewpoint_filter_scratch_bytes.argtypes = [i32, i64]
         d.lb2_viewpoint_filter_scratch_bytes.restype = C.c_size_t
         d.lb2_viewpoint_filter.argtypes = [vp, vp, vp, i32, vp, i64, C.c_double, vp, vp, vp]
+        f64 = C.c_double
+        for f in ("lb2_aggregate_window_scratch_bytes", "lb2_jitter_filter_scratch_bytes", "lb2_voxel_first_f64_scratch_bytes"):
+            getattr(d, f).argtypes = [i64]
+            getattr(d, f).restype = C.c_size_t
+        d.lb2_aggregate_window.argtypes = [vp, vp, vp, vp, i64, vp, i32, C.POINTER(f64), i64, vp, vp, vp]
+        d.lb2_jitter_filter.argtypes = [vp, vp, vp, vp, i64, f64, f64, f64, vp, vp, vp]
+        d.lb2_voxel_first_f64.argtypes = [vp, vp, vp, i64, f64, f64, vp, vp, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -456,6 +469,35 @@ class Handle:
         """rows of the fp64 (n, 3) `full` whose voxel_size cell holds a row of `part` -> `out` in order; d_out = [rows, status]"""
         self._check(self.dll.lb2_viewpoint_filter(self.hp, self._stream(), _ptr(part), int(part.shape[0]), _ptr(full), int(full.shape[0]),
                                                   float(voxel_size), _ptr(out), _ptr(d_out), _ptr(scratch)), "lb2_viewpoint_filter")
+
+    # -- refinement samples (lidiff_b200.datasets_refine) -------------------------------------------------------------------------
+    def aggregate_window_scratch(self, n: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_aggregate_window_scratch_bytes(int(n)))
+
+    def aggregate_window(self, points, labels, segments, nseg, undo12, split, out, d_out, scratch):
+        """label / range filter and the two rigid transforms of the window's (n, 4) fp32 `points` (int32 / uint32 `labels`) into the
+        fp64 (>= n, 3) `out`; `segments` = a device byte tensor of nseg Segment records; d_out = [rows kept, rows kept before `split`]"""
+        undo = (C.c_double * 12)(*[float(v) for v in undo12])
+        self._check(self.dll.lb2_aggregate_window(self.hp, self._stream(), _ptr(points), _ptr(labels), int(points.shape[0]), _ptr(segments),
+                                                  int(nseg), undo, int(split), _ptr(out), _ptr(d_out), _ptr(scratch)),
+                    "lb2_aggregate_window")
+
+    def jitter_filter_scratch(self, n: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_jitter_filter_scratch_bytes(int(n)))
+
+    def jitter_filter(self, points, randn, sigma, clip, max_range, out, d_count, scratch):
+        """rows p + clip(sigma * randn, +-clip) of the fp64 (n, 3) `points` within max_range -> `out` in order; d_count[0] = rows"""
+        self._check(self.dll.lb2_jitter_filter(self.hp, self._stream(), _ptr(points), _ptr(randn), int(points.shape[0]), float(sigma),
+                                               float(clip), float(max_range), _ptr(out), _ptr(d_count), _ptr(scratch)), "lb2_jitter_filter")
+
+    def voxel_first_f64_scratch(self, n: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_voxel_first_f64_scratch_bytes(int(n)))
+
+    def voxel_first_f64(self, points, voxel_size, max_range, out, d_out, scratch):
+        """first row of every floor(p / voxel_size) voxel of the fp64 (n, 3) `points`, within max_range -> `out` in row order;
+        d_out = [rows, status]"""
+        self._check(self.dll.lb2_voxel_first_f64(self.hp, self._stream(), _ptr(points), int(points.shape[0]), float(voxel_size),
+                                                 float(max_range), _ptr(out), _ptr(d_out), _ptr(scratch)), "lb2_voxel_first_f64")
 
 
 _LIB = None

@@ -79,6 +79,35 @@ __device__ __forceinline__ unsigned lb2_hash(unsigned long long k) {
     return (unsigned)k;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// voxel keys without a batch field (maps.cu, samples.cu): 3 x LB2_MAP_AXIS_BITS biased signed voxel indices, each in
+// [-2^20, 2^20); and the insert-or-find probe of an open-addressing key set built from them
+// ---------------------------------------------------------------------------------------------------
+#define LB2_MAP_AXIS_OFF (1 << (LB2_MAP_AXIS_BITS - 1))
+
+// f = floor(...) of one axis is a voxel index of the key range (NaN fails)
+template <class T>
+__device__ __forceinline__ bool lb2_map_cell_ok(T f) { return f >= -(T)LB2_MAP_AXIS_OFF && f < (T)LB2_MAP_AXIS_OFF; }
+
+// key with the next axis' voxel index appended (x first, then y, then z); `cell` has passed lb2_map_cell_ok
+__device__ __forceinline__ unsigned long long lb2_map_key_push(unsigned long long key, int cell) {
+    return (key << LB2_MAP_AXIS_BITS) | (unsigned long long)(unsigned)(cell + LB2_MAP_AXIS_OFF);
+}
+
+// slot of `key` in the key set keys[mask + 1] (linear probing from lb2_hash), inserted by CAS if absent; the set has a free slot
+__device__ __forceinline__ unsigned lb2_key_insert(unsigned long long* keys, unsigned mask, unsigned long long key) {
+    unsigned s = lb2_hash(key) & mask;
+    while (true) {
+        unsigned long long kk = keys[s];      // keys only go EMPTY -> key: a stale EMPTY falls through to the CAS
+        if (kk == LB2_KEY_EMPTY) {
+            kk = atomicCAS(keys + s, (unsigned long long)LB2_KEY_EMPTY, key);
+            if (kk == LB2_KEY_EMPTY) return s;
+        }
+        if (kk == key) return s;
+        s = (s + 1) & mask;
+    }
+}
+
 // row id of `key` in a built grid, or -1
 __device__ __forceinline__ int lb2_grid_lookup(const unsigned long long* __restrict__ keys,
                                                const int* __restrict__ rows, unsigned mask,

@@ -9,7 +9,6 @@
 #define MAP_THREADS  512
 #define MAP_ITEMS    4
 #define MAP_TILE     (MAP_THREADS * MAP_ITEMS)
-#define MAP_AXIS_OFF (1 << (LB2_MAP_AXIS_BITS - 1))
 
 struct MapScratch {        // carved out of the caller's scratch buffer
     int* slot_of;          // [n_cap] table slot claimed by point i, -1 = dropped (filtered or voxel already in the map)
@@ -52,8 +51,8 @@ __device__ __forceinline__ int map_point(const float4* __restrict__ pts, const u
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
         float f = floorf(div_mode == 0 ? __fdiv_rn(c[r], vs) : __fmul_rn(c[r], inv_vs));
-        if (!(f >= -(float)MAP_AXIS_OFF && f < (float)MAP_AXIS_OFF)) return 2;     // NaN fails too
-        key = (key << LB2_MAP_AXIS_BITS) | (unsigned long long)(unsigned)((int)f + MAP_AXIS_OFF);
+        if (!lb2_map_cell_ok(f)) return 2;
+        key = lb2_map_key_push(key, (int)f);
     }
     return 1;
 }
@@ -70,16 +69,7 @@ __global__ void __launch_bounds__(256) k_map_insert(const float4* __restrict__ p
     int slot = -1;
     if (st == 2) atomicOr(d_out + 1, 1);
     if (st == 1) {
-        unsigned mask = (unsigned)cap - 1u, s = lb2_hash(key) & mask;
-        while (true) {
-            unsigned long long kk = keys[s];      // keys only go EMPTY -> key: a stale EMPTY falls through to the CAS
-            if (kk == LB2_KEY_EMPTY) {
-                kk = atomicCAS(keys + s, (unsigned long long)LB2_KEY_EMPTY, key);
-                if (kk == LB2_KEY_EMPTY) break;
-            }
-            if (kk == key) break;
-            s = (s + 1) & mask;
-        }
+        unsigned s = lb2_key_insert(keys, (unsigned)cap - 1u, key);
         // rows are written only by k_map_emit of an earlier call; a slot without a row was created in this call
         if (vals[cap + s] < 0) {
             atomicMin(vals + s, i);

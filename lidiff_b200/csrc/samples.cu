@@ -1,7 +1,8 @@
 // Training / test samples of the diffusion network — stands behind lidiff/datasets/dataloader/SemanticKITTITemporal.py:82-105 (the
 // scan's label / range / height filter, the map crop about the scan pose and its transform into the scan frame) and
-// lidiff/utils/collations.py:44-51 (the 10 m viewpoint grid of the partial scan and the map points it includes).
-// Both calls are order-preserving compactions: a count pass, a scan of the block totals, and an emit pass that evaluates the same
+// lidiff/utils/collations.py:44-51 (the 10 m viewpoint grid of the partial scan and the map points it includes), and the refinement
+// network's samples (the end of this file).
+// Every call is an order-preserving compaction: a count pass, a scan of the block totals, and an emit pass that evaluates the same
 // inline predicate again and writes the kept rows at block offset + rank within the block.  Integer arithmetic decides every output
 // position, so the output is deterministic and in input order.  Rows are addressed with 64-bit indices (inputs up to 2^31 - 1 rows).
 #include "common.cuh"
@@ -319,4 +320,225 @@ extern "C" int lb2_viewpoint_filter(void* handle, void* stream, const double* pa
     LB2_POST_LAUNCH(h, "k_vp_insert");
     ViewpointSel sel{full, v.origin, v.keys, (unsigned)cap - 1u, voxel_size};
     return sel_compact(h, s, sel, n_full, v.boff, out, d_out);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// refinement samples — lidiff/utils/pcd_preprocess.py:78-129 (aggregate_pcds) and SemanticKITTITemporalAggr.py:69-99 (__getitem__)
+// ---------------------------------------------------------------------------------------------------
+// single block: d_out[0] = kept rows of [0, row) = the block offset of row's tile + the kept rows of that tile before `row`
+template <class Sel>
+__global__ void __launch_bounds__(SEL_THREADS) k_sel_rank_at(Sel sel, int64_t row, const long long* __restrict__ boff,
+                                                             int32_t* __restrict__ d_out) {
+    __shared__ int warp_cnt[SEL_WARPS];
+    int64_t base = row / SEL_TILE * SEL_TILE;
+    int cnt = 0;
+    for (int64_t i = base + threadIdx.x; i < row; i += SEL_THREADS) {
+        double3 w;
+        cnt += sel(i, w);
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) cnt += __shfl_down_sync(0xffffffffu, cnt, d);
+    if ((threadIdx.x & 31) == 0) warp_cnt[threadIdx.x >> 5] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        long long t = boff[row / SEL_TILE];
+        for (int k = 0; k < SEL_WARPS; ++k) t += warp_cnt[k];
+        d_out[0] = (int32_t)t;
+    }
+}
+
+// p' = ((m0 x + m1 y) + m2 z) + m3 per output axis in fp64, every operation rounded: numpy's
+// np.sum(np.expand_dims(hpoints, 2) * pose.T, axis=1) adds the four products of a row in column order (w = 1, so m3 * w = m3)
+__device__ __forceinline__ double3 rigid64(const double* __restrict__ m, double x, double y, double z) {
+    double c[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+        c[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[4 * r], x), __dmul_rn(m[4 * r + 1], y)), __dmul_rn(m[4 * r + 2], z)), m[4 * r + 3]);
+    return make_double3(c[0], c[1], c[2]);
+}
+
+struct AggregateSel {
+    const float4* pts;
+    const unsigned* labels;
+    const lb2_segment* seg;
+    int nseg;
+    double undo[12];
+
+    __device__ __forceinline__ bool operator()(int64_t i, double3& w) const {
+        unsigned l = __ldg(labels + i) & 0xFFFFu;
+        if (!(l < 252u)) return false;
+        float4 p = __ldg(pts + i);
+        float d = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(p.x, p.x), __fmul_rn(p.y, p.y)), __fmul_rn(p.z, p.z)));
+        if (!(d > 3.5f)) return false;                 // NaN fails, +-inf passes (numpy's comparison)
+        int lo = 0, hi = nseg - 1;                     // the last segment whose start is <= i (empty segments share a start)
+        while (lo < hi) {
+            int mid = (lo + hi + 1) >> 1;
+            if (__ldg(&seg[mid].start) <= i) lo = mid; else hi = mid - 1;
+        }
+        double m[12];
+#pragma unroll
+        for (int k = 0; k < 12; ++k) m[k] = __ldg(&seg[lo].m[k]);
+        double3 a = rigid64(m, (double)p.x, (double)p.y, (double)p.z);
+        w = rigid64(undo, a.x, a.y, a.z);
+        return true;
+    }
+};
+
+extern "C" size_t lb2_aggregate_window_scratch_bytes(int64_t n) { return lb2_select_points_scratch_bytes(n); }
+
+extern "C" int lb2_aggregate_window(void* handle, void* stream, const float* points, const uint32_t* labels, int64_t n,
+                                    const lb2_segment* segments, int32_t nseg, const double* undo, int64_t split, double* out,
+                                    int32_t* d_out, void* scratch) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h != nullptr, "handle");
+    LB2_REQUIRE(h, d_out != nullptr && undo != nullptr, "null d_out / undo");
+    LB2_REQUIRE(h, n >= 0 && n <= (int64_t)INT32_MAX, "n out of range (0 .. 2^31 - 1 rows)");
+    LB2_REQUIRE(h, nseg >= 1 && segments != nullptr, "at least one segment");
+    LB2_REQUIRE(h, split >= 0 && split <= n, "split out of range (0 .. n)");
+    LB2_REQUIRE(h, n == 0 || (points && labels && out && scratch), "null buffer");
+    cudaStream_t s = (cudaStream_t)stream;
+    if (cudaMemsetAsync(d_out, 0, 2 * sizeof(int32_t), s) != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "%s", "cudaMemsetAsync");
+    if (n == 0) return LB2_OK;
+    AggregateSel sel;
+    sel.pts = (const float4*)points; sel.labels = (const unsigned*)labels; sel.seg = segments; sel.nseg = nseg;
+    for (int k = 0; k < 12; ++k) sel.undo[k] = undo[k];
+    long long* boff = (long long*)scratch;
+    int rc = sel_compact(h, s, sel, n, boff, out, d_out);
+    if (rc != LB2_OK) return rc;
+    if (split == n) {                                  // every kept row comes before the split
+        if (cudaMemcpyAsync(d_out + 1, d_out, sizeof(int32_t), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+            return lb2_fail(h, LB2_ERR_CUDA, "%s", "cudaMemcpyAsync");
+        return LB2_OK;
+    }
+    k_sel_rank_at<<<1, SEL_THREADS, 0, s>>>(sel, split, boff, d_out + 1);
+    LB2_POST_LAUNCH(h, "k_sel_rank_at");
+    return LB2_OK;
+}
+
+// p + clip(sigma r, -clip, clip) (pcd_transforms.py:35-40: the scale, then numpy's clip = minimum(maximum(v, -clip), clip), then the
+// sum), kept where the fp64 distance sqrt((x^2 + y^2) + z^2) < r_max; NaN and inf rows fail the test
+struct JitterSel {
+    const double* p;
+    const double* r;
+    double sigma, clip, r_max;
+
+    __device__ __forceinline__ bool operator()(int64_t i, double3& w) const {
+        double c[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            double j = fmin(fmax(__dmul_rn(sigma, __ldg(r + 3 * i + k)), -clip), clip);
+            c[k] = __dadd_rn(j, __ldg(p + 3 * i + k));
+        }
+        double d = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(c[0], c[0]), __dmul_rn(c[1], c[1])), __dmul_rn(c[2], c[2])));
+        if (!(d < r_max)) return false;
+        w = make_double3(c[0], c[1], c[2]);
+        return true;
+    }
+};
+
+extern "C" size_t lb2_jitter_filter_scratch_bytes(int64_t n) { return lb2_select_points_scratch_bytes(n); }
+
+extern "C" int lb2_jitter_filter(void* handle, void* stream, const double* points, const double* randn, int64_t n, double sigma,
+                                 double clip, double max_range, double* out, int32_t* d_count, void* scratch) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h != nullptr, "handle");
+    LB2_REQUIRE(h, d_count != nullptr, "null d_count");
+    LB2_REQUIRE(h, n >= 0 && n <= (int64_t)INT32_MAX, "n out of range (0 .. 2^31 - 1 rows)");
+    LB2_REQUIRE(h, clip > 0.0, "clip must be > 0");
+    LB2_REQUIRE(h, n == 0 || (points && randn && out && scratch), "null buffer");
+    JitterSel sel{points, randn, sigma, clip, max_range};
+    return sel_compact(h, (cudaStream_t)stream, sel, n, (long long*)scratch, out, d_count);
+}
+
+// ---- first occurrence per voxel (ME.utils.sparse_quantize(p / voxel, return_index=True) on fp64 rows) ----
+struct VoxelFirstScratch {
+    unsigned long long* keys;   // [cap] voxel keys (lb2_map_key_push packing)
+    unsigned long long* claim;  // [cap] lowest row index of the slot's voxel
+    long long* boff;            // block offsets of the compaction
+};
+
+static int64_t vf_cap(int64_t n) { int64_t c = 16; while (c < 2 * n) c <<= 1; return c; }
+
+extern "C" size_t lb2_voxel_first_f64_scratch_bytes(int64_t n) {
+    return 2 * sel_align((size_t)vf_cap(n) * 8) + sel_align((size_t)sel_blocks(n > 0 ? n : 1) * sizeof(long long)) + 256;
+}
+
+static VoxelFirstScratch vf_carve(void* scratch, int64_t n) {
+    char* p = (char*)scratch;
+    size_t t = sel_align((size_t)vf_cap(n) * 8);
+    return VoxelFirstScratch{(unsigned long long*)p, (unsigned long long*)(p + t), (long long*)(p + 2 * t)};
+}
+
+// key of a row with finite coordinates: floor(p / voxel) per axis, the true fp64 quotient; false when an index is outside the key range
+__device__ __forceinline__ bool vf_key(double x, double y, double z, double voxel, unsigned long long& key) {
+    double c[3] = {x, y, z};
+    key = 0;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        double f = floor(__ddiv_rn(c[r], voxel));
+        if (!lb2_map_cell_ok(f)) return false;
+        key = lb2_map_key_push(key, (int)f);
+    }
+    return true;
+}
+
+// Rows with a NaN or inf coordinate are left out of the table: the reference gives them voxels of their own (no finite row floors to
+// them) and its distance test drops them afterwards, so leaving them out changes no output row.
+__global__ void k_vf_insert(const double* __restrict__ p, int64_t n, double voxel, unsigned long long* keys, unsigned long long* claim,
+                            unsigned mask, int32_t* __restrict__ d_out) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    double x = p[3 * i], y = p[3 * i + 1], z = p[3 * i + 2];
+    if (!(isfinite(x) && isfinite(y) && isfinite(z))) return;
+    unsigned long long key;
+    if (!vf_key(x, y, z, voxel, key)) {
+        atomicOr(d_out + 1, 1);
+        return;
+    }
+    atomicMin(claim + lb2_key_insert(keys, mask, key), (unsigned long long)i);
+}
+
+struct VoxelFirstSel {
+    const double* p;
+    const unsigned long long* keys;
+    const unsigned long long* claim;
+    unsigned mask;
+    double voxel, r_max;
+
+    __device__ __forceinline__ bool operator()(int64_t i, double3& w) const {
+        double x = p[3 * i], y = p[3 * i + 1], z = p[3 * i + 2];
+        if (!(isfinite(x) && isfinite(y) && isfinite(z))) return false;
+        unsigned long long key;
+        if (!vf_key(x, y, z, voxel, key)) return false;
+        unsigned s = lb2_hash(key) & mask;
+        while (keys[s] != key) s = (s + 1) & mask;        // inserted by k_vf_insert
+        if (claim[s] != (unsigned long long)i) return false;
+        double d = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));
+        if (!(d < r_max)) return false;
+        w = make_double3(x, y, z);
+        return true;
+    }
+};
+
+extern "C" int lb2_voxel_first_f64(void* handle, void* stream, const double* points, int64_t n, double voxel_size, double max_range,
+                                   double* out, int32_t* d_out, void* scratch) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h != nullptr, "handle");
+    LB2_REQUIRE(h, d_out != nullptr, "null d_out");
+    LB2_REQUIRE(h, n >= 0 && n <= (int64_t)INT32_MAX, "n out of range (0 .. 2^31 - 1 rows)");
+    LB2_REQUIRE(h, voxel_size > 0.0, "voxel_size must be > 0");
+    LB2_REQUIRE(h, n == 0 || (points && out && scratch), "null buffer");
+    cudaStream_t s = (cudaStream_t)stream;
+    if (cudaMemsetAsync(d_out, 0, 2 * sizeof(int32_t), s) != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "%s", "cudaMemsetAsync");
+    if (n == 0) return LB2_OK;
+    VoxelFirstScratch v = vf_carve(scratch, n);
+    int64_t cap = vf_cap(n);
+    // keys EMPTY and claims "none" are both all-ones: one clear of the two adjacent arrays
+    if (cudaMemsetAsync(v.keys, 0xFF, 2 * sel_align((size_t)cap * 8), s) != cudaSuccess)
+        return lb2_fail(h, LB2_ERR_CUDA, "%s", "cudaMemsetAsync");
+    unsigned mask = (unsigned)(cap - 1);
+    k_vf_insert<<<cdiv(n, 256), 256, 0, s>>>(points, n, voxel_size, v.keys, v.claim, mask, d_out);
+    LB2_POST_LAUNCH(h, "k_vf_insert");
+    VoxelFirstSel sel{points, v.keys, v.claim, mask, voxel_size, max_range};
+    return sel_compact(h, s, sel, n, v.boff, out, d_out);
 }

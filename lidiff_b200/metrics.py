@@ -299,3 +299,48 @@ def record_from_rows(rows: torch.Tensor) -> ScanRecord:
     c_gp = take(nt).view(np.int64).copy(); o += nt
     conf = take(3 * nv).view(np.uint64).reshape(nv, 3).copy()
     return ScanRecord(n_gt, n_pred, float(v[4]), float(v[5]), thr, c_pg, c_gp, vs, conf, float(v[6]), float(v[7]))
+
+
+def _nn_sq_dist(q: torch.Tensor, r: torch.Tensor) -> torch.Tensor:
+    """((q - r[idx])**2).sum(-1) in q's dtype, idx = the exact (fp64) nearest point of r to every row of q, lowest index on ties"""
+    _, idx = nn_distance(q, r, return_index=True, device=q.device)
+    return ((q - r[idx.long()]) ** 2).sum(-1)
+
+
+def chamfer_distance(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normals=None, weights=None, batch_reduction="mean",
+                     point_reduction="mean", norm=2):
+    """pytorch3d.loss.chamfer_distance (pytorch3d 0.7.1) with its defaults, on (B, P, 3) tensors on the GPU: (loss, None).
+
+    Every point's nearest neighbour in the other cloud is exact (lb2_pc_nn on fp64 coordinates, lowest index on ties), and its
+    squared distance is recomputed in the clouds' dtype as ((q - p[idx])**2).sum(-1); pytorch3d's fp32 brute force can pick the
+    other point of a near-tie, a few fp32 ulps apart (DESIGN.md §5).  The reductions are pytorch3d's torch ops in its order: the
+    per-cloud .sum(1), / lengths, .sum() / B, cham_x + cham_y.  Any other argument raises NotImplementedError."""
+    if any(a is not None for a in (x_lengths, y_lengths, x_normals, y_normals, weights)) or batch_reduction != "mean" or \
+            point_reduction != "mean" or norm != 2:
+        raise NotImplementedError("chamfer_distance: only pytorch3d's defaults (no lengths / normals / weights, mean reductions, "
+                                  "norm 2) are implemented")
+    if not (isinstance(x, torch.Tensor) and isinstance(y, torch.Tensor)) or x.dim() != 3 or y.dim() != 3 or x.shape[2] != 3 or \
+            y.shape[2] != 3:
+        raise ValueError(f"chamfer_distance: expected (B, P, 3) tensors, got {tuple(getattr(x, 'shape', ()))} and "
+                         f"{tuple(getattr(y, 'shape', ()))}")
+    if x.shape[0] != y.shape[0]:
+        raise ValueError("chamfer_distance: x and y must have the same batch dimension")
+    if x.shape[1] == 0 or y.shape[1] == 0:
+        raise ValueError("chamfer_distance: empty point cloud")
+    y = y.to(x.device)
+    n = x.shape[0]
+    with torch.no_grad():
+        cham_x = torch.stack([_nn_sq_dist(x[b], y[b]) for b in range(n)])          # (B, P1)
+        cham_y = torch.stack([_nn_sq_dist(y[b], x[b]) for b in range(n)])          # (B, P2)
+    x_lengths = torch.full((n,), x.shape[1], dtype=torch.int64, device=x.device)
+    y_lengths = torch.full((n,), y.shape[1], dtype=torch.int64, device=x.device)
+    cham_x = cham_x.sum(1)
+    cham_y = cham_y.sum(1)
+    cham_x /= x_lengths.clamp(min=1)
+    cham_y /= y_lengths.clamp(min=1)
+    cham_x = cham_x.sum()
+    cham_y = cham_y.sum()
+    div = max(n, 1)
+    cham_x /= div
+    cham_y /= div
+    return cham_x + cham_y, None

@@ -5,6 +5,20 @@ checkpoint callbacks; train.py:88-121) is out of scope (DESIGN.md §6) and raise
 from .core.lightning import LightningModule  # noqa: F401
 
 
+class LightningDataModule:
+    """A plain base class: the reference's data modules (lidiff/datasets/datasets_refine.py) subclass it and define their own
+    prepare_data / setup / *_dataloader methods."""
+
+    def __init__(self, *args, **kwargs):
+        pass
+
+    def prepare_data(self):
+        pass
+
+    def setup(self, stage=None):
+        pass
+
+
 class Trainer:
     def __init__(self, *a, **k):
         raise NotImplementedError("lidiff_b200 shims pytorch_lightning for inference only; training (SURVEY.md 8f-3) is not built")
