@@ -262,6 +262,20 @@ size_t lb2_packed_weight_bytes(int32_t kvol, int32_t cin, int32_t cout);
 int lb2_pack_weights(void* h, void* stream, const float* weight, int32_t kvol, int32_t cin, int32_t cout,
                      void* packed);
 
+/* Weight gradient of a sparse convolution (the backward of lb2_spconv_forward's product for one layer; the input gradient is that
+ * same forward on the adjoint map with transposed weights).  For every kernel offset k
+ *     dw[k] (cin x cout, fp32 row-major) = sum over o < m_out with nbr[k][o] >= 0 of x[nbr[k][o]]^T g[o]
+ * x (rows_in, cin) and g (m_out, cout) fp32; nbr [kvol][nbr_stride] as lb2_spconv_forward's, or NULL (identity, kvol 1).
+ * wgmma FP16x3 with the forward's split: x as an activation, g pre-scaled by a power of two 2^k (max|g| 2^k in [8192, 16384)) as a
+ * weight, so the forward's error model holds with x and g in the roles of x and w (chains of 60 MMA steps, one RN add per 320 rows).
+ * The rows are cut into a fixed number of chunks that depends on m_out only; each chunk's partial dw goes to scratch and a second
+ * kernel adds them in chunk order: no float atomics, the same bits from run to run.
+ * Shapes: kvol in {1, 8, 27}, cout in {32, 64, 96, 128, 256}, cin <= 512 and a multiple of 8 or below 8 (zero-padded); others
+ * LB2_ERR_UNSUP (lb2_spconv_wgrad_scratch_bytes returns 0).  scratch >= lb2_spconv_wgrad_scratch_bytes(kvol, cin, cout, m_out). */
+size_t lb2_spconv_wgrad_scratch_bytes(int32_t kvol, int32_t cin, int32_t cout, int32_t m_out);
+int lb2_spconv_wgrad(void* h, void* stream, const float* x, int32_t cin, const float* g, int32_t cout, int32_t m_out,
+                     const int32_t* nbr, int64_t nbr_stride, int32_t kvol, float* dw, void* scratch);
+
 /* ---- nearest partial-scan voxel — replaces pykeops argKmin(1) in MinkUNetDiff.match_part_to_full
  * (minkunet.py:403-418): idx[q] = argmin_j |cq - ck_j|^2 over [b*2*max, x, y, z], ties -> lowest j. */
 int lb2_nn_match(void* h, void* stream, const int32_t* q_coords, const int32_t* d_nq, int32_t nq_cap,
@@ -371,6 +385,12 @@ size_t lb2_pc_tree_bytes(int32_t n_cap);
 size_t lb2_pc_nn_scratch_bytes(int32_t nq_cap);
 int lb2_pc_tree_build(void* h, void* stream, const double* pts, int32_t n, void* tree);
 int lb2_pc_nn(void* h, void* stream, const double* q, int32_t nq, const void* tree, double* dist, int32_t* idx, void* scratch);
+
+/* Deterministic segmented sum (the backward of a row gather, e.g. the Chamfer loss' x[idx]):
+ *     out[s][j] = sum over i in [offsets[s], offsets[s + 1]) of values[order[i]][j], added in ascending i
+ * values (rows, c) fp32, or fp64 with f64 = 1; order int64 (NULL = identity); offsets int64[nseg + 1]; out (nseg, c). */
+int lb2_segment_sum(void* h, void* stream, const void* values, int32_t f64, const int64_t* order, const int64_t* offsets,
+                    int64_t nseg, int32_t c, void* out);
 
 /* Point normals as open3d 0.17's PointCloud.estimate_normals() computes them (KDTreeSearchParamKNN(30), fast_normal_computation;
  * tools/diff_completion_pipeline.py:204-212), in two steps over a tree from lb2_pc_tree_build(pts, n):

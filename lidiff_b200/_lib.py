@@ -73,6 +73,7 @@ EXPORTS = [
     "lb2_select_points_scratch_bytes", "lb2_select_points", "lb2_viewpoint_filter_scratch_bytes", "lb2_viewpoint_filter",
     "lb2_aggregate_window_scratch_bytes", "lb2_aggregate_window", "lb2_jitter_filter_scratch_bytes", "lb2_jitter_filter",
     "lb2_voxel_first_f64_scratch_bytes", "lb2_voxel_first_f64",
+    "lb2_spconv_wgrad_scratch_bytes", "lb2_spconv_wgrad", "lb2_segment_sum",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -190,6 +191,10 @@ class Lib:
         d.lb2_aggregate_window.argtypes = [vp, vp, vp, vp, i64, vp, i32, C.POINTER(f64), i64, vp, vp, vp]
         d.lb2_jitter_filter.argtypes = [vp, vp, vp, vp, i64, f64, f64, f64, vp, vp, vp]
         d.lb2_voxel_first_f64.argtypes = [vp, vp, vp, i64, f64, f64, vp, vp, vp]
+        d.lb2_spconv_wgrad_scratch_bytes.argtypes = [i32, i32, i32, i32]
+        d.lb2_spconv_wgrad_scratch_bytes.restype = C.c_size_t
+        d.lb2_spconv_wgrad.argtypes = [vp, vp, vp, i32, vp, i32, i32, vp, i64, i32, vp, vp]
+        d.lb2_segment_sum.argtypes = [vp, vp, vp, i32, vp, vp, i64, i32, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -313,6 +318,22 @@ class Handle:
         out = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         self._check(self.dll.lb2_pack_weights(self.hp, self._stream(), _ptr(w), kvol, cin, cout, _ptr(out)), "lb2_pack_weights")
         return out
+
+    def spconv_wgrad(self, x, g, nbr, kvol, dw):
+        """dw (kvol, cin, cout) fp32 = per offset k: sum over output rows o of x[nbr[k][o]]^T g[o] (nbr None: identity, kvol 1)"""
+        cin, (m_out, cout) = x.shape[1], g.shape
+        nbytes = int(self.dll.lb2_spconv_wgrad_scratch_bytes(int(kvol), int(cin), int(cout), int(m_out)))
+        if nbytes == 0:
+            raise RuntimeError(f"lb2_spconv_wgrad: no kernel for kvol {kvol}, {cin} -> {cout} channels")
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        self._check(self.dll.lb2_spconv_wgrad(self.hp, self._stream(), _ptr(x), int(cin), _ptr(g), int(cout), int(m_out), _ptr(nbr),
+                                              int(nbr.stride(0)) if nbr is not None else 0, int(kvol), _ptr(dw), _ptr(scratch)),
+                    "lb2_spconv_wgrad")
+
+    def segment_sum(self, values, order, offsets, out):
+        """out[s] = sum of values[order[i]] over i in [offsets[s], offsets[s + 1]), in ascending i (order None: identity)"""
+        self._check(self.dll.lb2_segment_sum(self.hp, self._stream(), _ptr(values), int(values.dtype == torch.float64), _ptr(order),
+                                             _ptr(offsets), int(offsets.shape[0] - 1), int(values.shape[1]), _ptr(out)), "lb2_segment_sum")
 
     # -- misc ----------------------------------------------------------------------------------------
     def nn_match(self, q, d_nq, nq_cap, k, d_nk, nk_cap, batch_scale, idx):

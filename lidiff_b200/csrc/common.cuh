@@ -16,8 +16,8 @@ struct Lb2Handle {
 };
 
 // kernels that need more than 48 KB of dynamic shared memory: the attribute is per-device state, the handle is per device
-// (LB2_K_TC and LB2_K_SCATTER: one bit per instantiation, N = 32, 64, 96, 128)
-enum { LB2_K_TC = 0, LB2_K_SCATTER = 4, LB2_K_NN_TABLE = 8, LB2_K_FPS_CLUSTER = 9 };
+// (LB2_K_TC and LB2_K_SCATTER: one bit per instantiation, N = 32, 64, 96, 128; LB2_K_WGRAD: N = 32, 64)
+enum { LB2_K_TC = 0, LB2_K_SCATTER = 4, LB2_K_NN_TABLE = 8, LB2_K_FPS_CLUSTER = 9, LB2_K_WGRAD = 10 };
 template <class K>
 static inline cudaError_t lb2_configure_smem(Lb2Handle* h, int bit, K kernel, int bytes) {
     if (h->configured & (1u << bit)) return cudaSuccess;

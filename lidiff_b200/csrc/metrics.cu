@@ -730,3 +730,33 @@ extern "C" int lb2_dist_stats(void* handle, void* stream, const double* dist, in
     LB2_POST_LAUNCH(h, "k_ds_final");
     return LB2_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------
+// segment_sum: out[s] = sum of values[order[i]] over i in [offsets[s], offsets[s + 1]), added in ascending i (one warp per segment,
+// lanes over channels).  The backward of a row gather (the Chamfer loss' x[idx], slice()) without atomics.
+// ---------------------------------------------------------------------------------------------------
+template <class T>
+__global__ void k_segment_sum(const T* __restrict__ values, const int64_t* __restrict__ order, const int64_t* __restrict__ offsets,
+                              int64_t nseg, int32_t c, T* __restrict__ out) {
+    const int64_t seg = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (seg >= nseg) return;
+    const int64_t b = offsets[seg], e = offsets[seg + 1];
+    for (int j = lane; j < c; j += 32) {
+        T s = 0;
+        for (int64_t i = b; i < e; ++i) s += values[(order ? order[i] : i) * c + j];
+        out[seg * c + j] = s;
+    }
+}
+
+extern "C" int lb2_segment_sum(void* handle, void* stream, const void* values, int32_t f64, const int64_t* order,
+                               const int64_t* offsets, int64_t nseg, int32_t c, void* out) {
+    Lb2Handle* h = (Lb2Handle*)handle;
+    LB2_REQUIRE(h, h && values && offsets && out && nseg >= 0 && c > 0, "segment_sum");
+    if (nseg == 0) return LB2_OK;
+    const unsigned grid = cdiv(nseg * 32, 256);
+    if (f64) k_segment_sum<double><<<grid, 256, 0, (cudaStream_t)stream>>>((const double*)values, order, offsets, nseg, c, (double*)out);
+    else k_segment_sum<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)values, order, offsets, nseg, c, (float*)out);
+    LB2_POST_LAUNCH(h, "k_segment_sum");
+    return LB2_OK;
+}

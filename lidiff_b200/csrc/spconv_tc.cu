@@ -422,26 +422,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_tc(const Params p) {
 
 // ---- weight packing: (kvol, cin, cout) fp32 -> [256 B header][per (k, chunk): hi tile | lo tile], each tile cout rows
 // x 128 B in the K-major SWIZZLE_128B image, channels beyond cin zero-filled.  Values are W * 2^k with k chosen so
-// that max|W| * 2^k lies in [8192, 16384); header[1] = 2^-k is applied to the accumulator in the epilogue. ---------
-__global__ void k_weight_absmax(const float* __restrict__ w, long long n, unsigned* __restrict__ header) {
-    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    float m = 0.f;
-    for (; t < n; t += (long long)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(w[t]));
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0) atomicMax(header, __float_as_uint(m));      // non-negative floats order like uints
-}
-
-__device__ __forceinline__ float weight_scale(unsigned max_bits) {
-    const float m = __uint_as_float(max_bits);
-    if (!(m > 0.f) || !isfinite(m)) return 1.f;
-    int e;
-    frexpf(m, &e);                         // m = f * 2^e, f in [0.5, 1)
-    // m * scale in [8192, 16384); below m = 2^-113 it stops at 2^126, so that the scale and header[1] = 2^-126 stay finite, nonzero
-    // and normal (nothing depends on how the build treats fp32 subnormals)
-    return ldexpf(1.f, min(14 - e, 126));
-}
-
+// that max|W| * 2^k lies in [8192, 16384) (k_weight_absmax, weight_scale); header[1] = 2^-k is applied to the accumulator in the
+// epilogue. ---------
 __global__ void k_pack_weights(const float* __restrict__ w, int kvol, int cin, int cout, int nchunks, unsigned char* __restrict__ out) {
     const long long total = (long long)kvol * nchunks * cout * KC;
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;

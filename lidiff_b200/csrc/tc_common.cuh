@@ -208,6 +208,28 @@ __device__ __forceinline__ float4 load_residual4(const float* res, const void* r
     return make_float4(h0.x + l0.x, h0.y + l0.y, h1.x + l1.x, h1.y + l1.y);
 }
 
+// power-of-two pre-scale of the operand that the FP16x3 product splits like a weight (the packed weights of the forward, the output
+// gradient of the weight gradient): header[0] = max|v| as float bits (atomicMax, the caller zeroes it first), and
+// v * weight_scale(header[0]) has its largest magnitude in [8192, 16384)
+static __global__ void k_weight_absmax(const float* __restrict__ w, long long n, unsigned* __restrict__ header) {
+    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    float m = 0.f;
+    for (; t < n; t += (long long)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(w[t]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(header, __float_as_uint(m));      // non-negative floats order like uints
+}
+
+__device__ __forceinline__ float weight_scale(unsigned max_bits) {
+    const float m = __uint_as_float(max_bits);
+    if (!(m > 0.f) || !isfinite(m)) return 1.f;
+    int e;
+    frexpf(m, &e);                         // m = f * 2^e, f in [0.5, 1)
+    // m * scale in [8192, 16384); below m = 2^-113 it stops at 2^126, so that the scale and header[1] = 2^-126 stay finite, nonzero
+    // and normal (nothing depends on how the build treats fp32 subnormals)
+    return ldexpf(1.f, min(14 - e, 126));
+}
+
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }

@@ -134,11 +134,56 @@ class TensorField:
         cm = self.coordinate_manager
         if 1 not in cm.levels:
             cm.insert_field(self._C)
-        lvl = cm.levels[1]
-        n, c = self._F.shape
-        out = torch.empty((lvl.n, c), dtype=torch.float32, device=self.device)
-        cm.h.voxel_mean(self._F, cm.field_inverse, n, c, None, lvl.n, out, cm.h.voxel_mean_scratch(lvl.n, c))
+        if torch.is_grad_enabled() and self._F.requires_grad:
+            out = _VoxelMean.apply(self._F, cm)
+        else:
+            out = _voxel_mean(self._F, cm)
         return SparseTensor(out, coordinate_manager=cm, tensor_stride=1)
+
+
+def _voxel_mean(F, cm):
+    lvl = cm.levels[1]
+    n, c = F.shape
+    out = torch.empty((lvl.n, c), dtype=torch.float32, device=F.device)
+    cm.h.voxel_mean(F, cm.field_inverse, n, c, None, lvl.n, out, cm.h.voxel_mean_scratch(lvl.n, c))
+    return out
+
+
+def _gather(src, cm, n):
+    out = torch.empty((n, src.shape[1]), dtype=torch.float32, device=src.device)
+    cm.h.gather_rows(src, cm.field_inverse, n, src.shape[1], out)
+    return out
+
+
+class _VoxelMean(torch.autograd.Function):
+    """TensorField.sparse(): the mean of each voxel's points; backward: every point gets its voxel's gradient / member count"""
+
+    @staticmethod
+    def forward(ctx, F, cm):
+        ctx.cm, ctx.n = cm, F.shape[0]
+        return _voxel_mean(F, cm)
+
+    @staticmethod
+    def backward(ctx, grad):
+        cm = ctx.cm
+        count = torch.bincount(cm.field_inverse.long(), minlength=grad.shape[0]).to(grad.dtype)
+        return _gather((grad / count[:, None]).contiguous(), cm, ctx.n), None
+
+
+class _Slice(torch.autograd.Function):
+    """SparseTensor.slice(): every point takes its voxel's row; backward: per voxel, the sum of its points' gradients in point
+    order (rowsum.index_sum: no atomics, the same bits on every run)"""
+
+    @staticmethod
+    def forward(ctx, F, cm, n):
+        ctx.cm = cm
+        return _gather(F, cm, n)
+
+    @staticmethod
+    def backward(ctx, grad):
+        from .rowsum import index_sum
+        cm = ctx.cm
+        return index_sum(grad.float(), cm.field_inverse, cm.levels[1].n), None, None
 
 
 class SparseTensor:
@@ -196,9 +241,11 @@ class SparseTensor:
         if field.coordinate_manager is not self.coordinate_manager or self.tensor_stride != 1:
             raise RuntimeError("slice: tensor field and sparse tensor must share the stride-1 coordinate map")
         cm = self.coordinate_manager
-        n, c = field.F.shape[0], self._F.shape[1]
-        out = torch.empty((n, c), dtype=torch.float32, device=self.device)
-        cm.h.gather_rows(self._F.contiguous(), cm.field_inverse, n, c, out)
+        n = field.F.shape[0]
+        if torch.is_grad_enabled() and self._F.requires_grad:
+            out = _Slice.apply(self._F.contiguous(), cm, n)
+        else:
+            out = _gather(self._F.contiguous(), cm, n)
         return TensorField(out, field.C, coordinate_manager=cm)
 
 
@@ -267,11 +314,22 @@ class _ConvBase(nn.Module):
             ts_out = ts // self.stride
         else:
             ts_out = ts * self.stride
+        if torch.is_grad_enabled() and (F.requires_grad or self.kernel.requires_grad):
+            out = _ConvFn.apply(F, self.kernel, self, cm, ts, ts_out)
+        else:
+            out = self._conv(F, cm, ts, ts_out)
+        return SparseTensor(out, coordinate_manager=cm, tensor_stride=ts_out)
+
+    def _map(self, cm, ts):
+        """the forward kernel map (kvol, rows out), or None for the 1x1 identity"""
+        if self.kernel.dim() == 3 and not (self.kernel_volume == 1):
+            return cm.kernel_map(ts, self.kernel_size, self.stride, self.transposed)
+        return None
+
+    def _conv(self, F, cm, ts, ts_out):
         lout = cm.level(ts_out)
         W = self.kernel
-        nbr = None
-        if W.dim() == 3 and not (self.kernel_volume == 1):
-            nbr = cm.kernel_map(ts, self.kernel_size, self.stride, self.transposed)
+        nbr = self._map(cm, ts)
         out = torch.empty((lout.n, self.out_channels), dtype=torch.float32, device=F.device)
         d = ConvDesc()
         d.c1, d.c2, d.cout, d.kvol = self.in_channels, 0, self.out_channels, self.kernel_volume
@@ -284,7 +342,97 @@ class _ConvBase(nn.Module):
         d.io[0] = ConvIO(F.data_ptr(), None, None, out.data_ptr(), None, None, None)
         if lout.n > 0:
             cm.h.spconv(d, getattr(self, "algo", _lib.ALGO_AUTO))
-        return SparseTensor(out, coordinate_manager=cm, tensor_stride=ts_out)
+        return out
+
+    # ---- backward ------------------------------------------------------------------------------------------------------------
+    def _adjoint(self, cm, ts, ts_out):
+        """(map, weight transform) of the input gradient: dX = conv(G) on the adjoint map with the transformed kernel.
+        3x3x3 stride 1: the same map, offset k <- 26 - k (the map is symmetric: nbr[k][o] = i <=> nbr[26 - k][i] = o), W[26 - k]^T.
+        k2 s2 (fine -> coarse): the transposed map coarse -> fine, W[k]^T; a transposed convolution: the strided map, W[k]^T.
+        1x1: the identity, W^T."""
+        W = self.kernel.detach()
+        if W.dim() == 2:
+            return None, W.t()[None]
+        if self.kernel_volume == 1:
+            return None, W.transpose(1, 2)
+        if self.kernel_size == 3 and self.stride == 1:
+            return cm.kernel_map(ts, 3, 1, False), W.flip(0).transpose(1, 2)
+        if self.transposed:
+            return cm.kernel_map(ts_out, self.kernel_size, self.stride, False), W.transpose(1, 2)
+        return cm.kernel_map(ts_out, self.kernel_size, self.stride, True), W.transpose(1, 2)
+
+    def _adjoint_packs(self, h, Wt):
+        """transformed kernel slices of at most 256 (or 128) output channels, packed for the tensor cores and cached until the
+        parameter changes (an optimizer step bumps its version): [(c0, c1, weight, packed)]"""
+        W = self.kernel
+        key = (W.data_ptr(), W._version)
+        if getattr(self, "_adj_key", None) != key:
+            cin = Wt.shape[2]
+            # the forward kernel takes Cout <= 128 or exactly 256: 384 runs as 256 + 128, 192 as 128 + 64
+            cuts = {384: (0, 256, 384), 192: (0, 128, 192)}.get(cin, (0, cin))
+            packs = []
+            for c0, c1 in zip(cuts[:-1], cuts[1:]):
+                w = Wt[:, :, c0:c1].contiguous()
+                pk = h.pack_weights(w)
+                if pk is None:
+                    raise RuntimeError(f"{type(self).__name__}({self.in_channels}, {self.out_channels}): no tensor-core kernel for the "
+                                       f"input gradient's {c1 - c0} output channels")
+                packs.append((c0, c1, w, pk))
+            self._adj, self._adj_key = packs, key
+        return self._adj
+
+    def _input_grad(self, G, cm, ts, ts_out):
+        nbr, Wt = self._adjoint(cm, ts, ts_out)
+        lin = cm.level(ts)
+        # the output gradient is the activation operand of the FP16x3 product, whose split has an absolute floor of 2^-25: scale it
+        # by a power of two so that its largest magnitude lies in [8192, 16384), as the packed weights are (exact both ways)
+        amax = G.abs().amax()
+        e = torch.frexp(amax).exponent
+        scale = torch.where(torch.isfinite(amax) & (amax > 0), torch.ldexp(torch.ones_like(amax), (14 - e).clamp(max=126)),
+                            torch.ones_like(amax))
+        Gs = (G * scale).contiguous()
+        parts = []
+        for c0, c1, w, pk in self._adjoint_packs(cm.h, Wt):
+            out = torch.empty((lin.n, c1 - c0), dtype=torch.float32, device=G.device)
+            d = ConvDesc()
+            d.c1, d.c2, d.cout, d.kvol = self.out_channels, 0, c1 - c0, w.shape[0]
+            d.weight, d.weight_packed = w.data_ptr(), pk.data_ptr()
+            d.relu = 0
+            d.nbr = nbr.data_ptr() if nbr is not None else None
+            d.nbr_stride = lin.n
+            d.mout_cap, d.npass = lin.n, 1
+            d.io[0] = ConvIO(Gs.data_ptr(), None, None, out.data_ptr(), None, None, None)
+            if lin.n > 0:
+                cm.h.spconv(d, _lib.ALGO_TC)
+            parts.append(out)
+        out = parts[0] if len(parts) == 1 else torch.cat(parts, 1)
+        return out / scale
+
+    def _weight_grad(self, F, G, cm, ts):
+        nbr = self._map(cm, ts)
+        dw = torch.empty((self.kernel_volume, self.in_channels, self.out_channels), dtype=torch.float32, device=G.device)
+        cm.h.spconv_wgrad(F, G, nbr, self.kernel_volume, dw)
+        return dw.reshape(self.kernel.shape)
+
+
+class _ConvFn(torch.autograd.Function):
+    """a sparse convolution with its gradients: dX on the adjoint map (the forward kernels, _ConvBase._input_grad), dW from
+    lb2_spconv_wgrad.  The forward is the no-grad call itself, so its values are the same bits."""
+
+    @staticmethod
+    def forward(ctx, F, W, layer, cm, ts, ts_out):
+        ctx.save_for_backward(F)
+        ctx.layer, ctx.cm, ctx.ts, ctx.ts_out = layer, cm, ts, ts_out
+        return layer._conv(F, cm, ts, ts_out)
+
+    @staticmethod
+    def backward(ctx, G):
+        (F,) = ctx.saved_tensors
+        layer, cm = ctx.layer, ctx.cm
+        G = G.contiguous()
+        dF = layer._input_grad(G, cm, ctx.ts, ctx.ts_out) if ctx.needs_input_grad[0] else None
+        dW = layer._weight_grad(F, G, cm, ctx.ts) if ctx.needs_input_grad[1] else None
+        return dF, dW, None, None, None, None
 
 
 class MinkowskiConvolution(_ConvBase):

@@ -22,6 +22,7 @@ import scipy.integrate
 import torch
 
 from . import _lib
+from .rowsum import GatherRows
 
 MAX_RANGE = 50.0                        # histogram range [-MAX_RANGE, MAX_RANGE] on every axis (metrics.py:88)
 JSD_VOXEL = 0.5                         # histogram_metrics.py:48-49
@@ -302,9 +303,11 @@ def record_from_rows(rows: torch.Tensor) -> ScanRecord:
 
 
 def _nn_sq_dist(q: torch.Tensor, r: torch.Tensor) -> torch.Tensor:
-    """((q - r[idx])**2).sum(-1) in q's dtype, idx = the exact (fp64) nearest point of r to every row of q, lowest index on ties"""
-    _, idx = nn_distance(q, r, return_index=True, device=q.device)
-    return ((q - r[idx.long()]) ** 2).sum(-1)
+    """((q - r[idx])**2).sum(-1) in q's dtype, idx = the exact (fp64) nearest point of r to every row of q, lowest index on ties.
+    Differentiable in q and r; the gradient of r[idx] is summed per row of r in query order (rowsum.GatherRows), without atomics."""
+    with torch.no_grad():
+        _, idx = nn_distance(q, r, return_index=True, device=q.device)
+    return ((q - GatherRows.apply(r, idx.long())) ** 2).sum(-1)
 
 
 def chamfer_distance(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normals=None, weights=None, batch_reduction="mean",
@@ -314,7 +317,10 @@ def chamfer_distance(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_nor
     Every point's nearest neighbour in the other cloud is exact (lb2_pc_nn on fp64 coordinates, lowest index on ties), and its
     squared distance is recomputed in the clouds' dtype as ((q - p[idx])**2).sum(-1); pytorch3d's fp32 brute force can pick the
     other point of a near-tie, a few fp32 ulps apart (DESIGN.md §5).  The reductions are pytorch3d's torch ops in its order: the
-    per-cloud .sum(1), / lengths, .sum() / B, cham_x + cham_y.  Any other argument raises NotImplementedError."""
+    per-cloud .sum(1), / lengths, .sum() / B, cham_x + cham_y.  Any other argument raises NotImplementedError.
+
+    The loss is differentiable in x and y: the neighbour indices are fixed by the forward (as pytorch3d's backward uses its knn
+    indices), and the gradient that the cham_y term sends to x[idx_y] is summed per point of x in a fixed order."""
     if any(a is not None for a in (x_lengths, y_lengths, x_normals, y_normals, weights)) or batch_reduction != "mean" or \
             point_reduction != "mean" or norm != 2:
         raise NotImplementedError("chamfer_distance: only pytorch3d's defaults (no lengths / normals / weights, mean reductions, "
@@ -329,9 +335,8 @@ def chamfer_distance(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_nor
         raise ValueError("chamfer_distance: empty point cloud")
     y = y.to(x.device)
     n = x.shape[0]
-    with torch.no_grad():
-        cham_x = torch.stack([_nn_sq_dist(x[b], y[b]) for b in range(n)])          # (B, P1)
-        cham_y = torch.stack([_nn_sq_dist(y[b], x[b]) for b in range(n)])          # (B, P2)
+    cham_x = torch.stack([_nn_sq_dist(x[b], y[b]) for b in range(n)])          # (B, P1)
+    cham_y = torch.stack([_nn_sq_dist(y[b], x[b]) for b in range(n)])          # (B, P2)
     x_lengths = torch.full((n,), x.shape[1], dtype=torch.int64, device=x.device)
     y_lengths = torch.full((n,), y.shape[1], dtype=torch.int64, device=x.device)
     cham_x = cham_x.sum(1)
