@@ -181,7 +181,9 @@ __global__ void __launch_bounds__(THREADS, 1) k_spconv_wgrad(const Params p) {
         if (in_group > 0) {
             wgmma_wait<0>();
             reg_fence(acc);
-            if (lane == 0) mbar_arrive(empty(prev_s));
+            // an empty stage after the group's last live one has already released it (prev_s = -1); empty(-1) would be the
+            // address of full(MAX_STAGES - 1)
+            if (prev_s >= 0 && lane == 0) mbar_arrive(empty(prev_s));
 #pragma unroll
             for (int j = 0; j < NC / 2; ++j) tot[j] = __fadd_rn(tot[j], acc[j]);
         }
@@ -244,18 +246,19 @@ extern "C" int lb2_spconv_wgrad(void* handle, void* stream, const float* x, int3
                                 const int32_t* nbr, int64_t nbr_stride, int32_t kvol, float* dw, void* scratch) {
     using namespace tc::wgrad;
     Lb2Handle* h = (Lb2Handle*)handle;
-    LB2_REQUIRE(h, h && x && g && dw && scratch, "spconv_wgrad null");
+    LB2_REQUIRE(h, h && dw && scratch, "spconv_wgrad null");
     LB2_REQUIRE(h, m_out >= 0, "m_out");
-    LB2_REQUIRE(h, nbr != nullptr || kvol == 1, "identity map only for kvol == 1");
-    LB2_REQUIRE(h, nbr == nullptr || nbr_stride >= m_out, "nbr_stride");
     if (!shape_ok(kvol, cin, cout))
         return lb2_fail(h, LB2_ERR_UNSUP, "spconv_wgrad: no tensor-core kernel for this (kvol, cin, cout)%s", "");
     cudaStream_t s = (cudaStream_t)stream;
     const long long total = (long long)kvol * cin * cout;
-    if (m_out == 0) {
+    if (m_out == 0) {                    // no rows: G and the map are empty (an empty tensor may have no data pointer)
         if (cudaMemsetAsync(dw, 0, (size_t)total * sizeof(float), s) != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "spconv_wgrad memset%s", "");
         return LB2_OK;
     }
+    LB2_REQUIRE(h, x && g, "spconv_wgrad null");
+    LB2_REQUIRE(h, nbr != nullptr || kvol == 1, "identity map only for kvol == 1");
+    LB2_REQUIRE(h, nbr == nullptr || nbr_stride >= m_out, "nbr_stride");
     unsigned* header = (unsigned*)scratch;
     if (cudaMemsetAsync(header, 0, tc::PACK_HEADER, s) != cudaSuccess) return lb2_fail(h, LB2_ERR_CUDA, "spconv_wgrad memset%s", "");
     const long long ng = (long long)m_out * cout;

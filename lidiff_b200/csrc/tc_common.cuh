@@ -209,12 +209,17 @@ __device__ __forceinline__ float4 load_residual4(const float* res, const void* r
 }
 
 // power-of-two pre-scale of the operand that the FP16x3 product splits like a weight (the packed weights of the forward, the output
-// gradient of the weight gradient): header[0] = max|v| as float bits (atomicMax, the caller zeroes it first), and
-// v * weight_scale(header[0]) has its largest magnitude in [8192, 16384)
+// gradient of the weight gradient): header[0] = max|v| over the finite v as float bits (atomicMax, the caller zeroes it first), and
+// v * weight_scale(header[0]) has its largest finite magnitude in [8192, 16384).  A NaN or +-inf element is skipped: it makes the
+// outputs that read it non-finite whatever the scale, and taking its magnitude (fmaxf skips NaN, but +inf wins) would leave every
+// other element unscaled, its low half lost below the fp16 subnormal range.
 static __global__ void k_weight_absmax(const float* __restrict__ w, long long n, unsigned* __restrict__ header) {
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     float m = 0.f;
-    for (; t < n; t += (long long)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(w[t]));
+    for (; t < n; t += (long long)gridDim.x * blockDim.x) {
+        const float a = fabsf(w[t]);
+        if (isfinite(a)) m = fmaxf(m, a);
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) atomicMax(header, __float_as_uint(m));      // non-negative floats order like uints

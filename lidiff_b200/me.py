@@ -287,7 +287,8 @@ class _ConvBase(nn.Module):
         with torch.no_grad():
             n = (self.out_channels if self.transposed else self.in_channels) * self.kernel_volume
             stdv = 1.0 / math.sqrt(n)
-            self.kernel.data.uniform_(-stdv, stdv)
+            # not through .data: that write would leave the parameter's version, and with it the packed-weight caches, unchanged
+            self.kernel.uniform_(-stdv, stdv)
 
     def _packed_weight(self, h):
         """tensor-core image of the kernel (fp16 hi/lo, wgmma layout), cached until the parameter changes"""
@@ -385,8 +386,11 @@ class _ConvBase(nn.Module):
         nbr, Wt = self._adjoint(cm, ts, ts_out)
         lin = cm.level(ts)
         # the output gradient is the activation operand of the FP16x3 product, whose split has an absolute floor of 2^-25: scale it
-        # by a power of two so that its largest magnitude lies in [8192, 16384), as the packed weights are (exact both ways)
-        amax = G.abs().amax()
+        # by a power of two so that its largest magnitude lies in [8192, 16384), as the packed weights are (exact both ways).  Only
+        # finite elements count, as in k_weight_absmax: a NaN or inf row makes the rows that read it non-finite whatever the scale,
+        # and must not leave the others unscaled
+        Ga = G.abs()
+        amax = torch.where(torch.isfinite(Ga), Ga, torch.zeros_like(Ga)).amax()
         e = torch.frexp(amax).exponent
         scale = torch.where(torch.isfinite(amax) & (amax > 0), torch.ldexp(torch.ones_like(amax), (14 - e).clamp(max=126)),
                             torch.ones_like(amax))

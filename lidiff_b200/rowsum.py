@@ -17,6 +17,8 @@ def index_sum(values: torch.Tensor, idx: torch.Tensor, n: int) -> torch.Tensor:
     out = torch.empty((n, values.shape[1]), dtype=values.dtype, device=values.device)
     if n == 0:
         return out
+    if values.shape[0] == 0:            # no rows: every sum is empty (and an empty tensor has no data pointer to pass)
+        return out.zero_()
     idx = idx.long()
     order = torch.sort(idx, stable=True).indices
     offsets = torch.zeros(n + 1, dtype=torch.int64, device=values.device)

@@ -174,3 +174,27 @@ def test_non_finite_rows_reach_exactly_their_outputs(c, algo, use_h):
     assert bad.any()
     assert torch.equal(~torch.isfinite(y), bad), "non-finite outputs differ from the fp64 reference's"
     assert sn.same_bits(y[~bad], y0[~bad]), "a row that does not read the non-finite rows changed"
+
+
+@pytest.mark.parametrize("use_h", [False, True])
+@pytest.mark.parametrize("value", [float("inf"), float("nan")])
+@pytest.mark.parametrize("c", [(64, 0, 64, 27, 0, False), (128, 64, 256, 27, 0, False)], ids=sn.case_id)
+def test_non_finite_weight_reaches_only_its_output_channel(c, value, use_h):
+    """one +inf or NaN weight W[k][i][j]: the packer's pre-scale follows the largest finite weight, so every output outside channel
+    j has the bits of a run with that weight zeroed, and channel j is non-finite wherever the fp64 reference is.  An output row
+    without neighbour k multiplies the weight by a zero-filled row (0 * inf = NaN), so channel j may be non-finite there too."""
+    h = H()
+    X, W = sn.case_operands(c)
+    k, i, j = 5, 7, c[2] // 3
+    W0 = W.clone()
+    W0[k, i, j] = 0
+    Wb = W0.clone()
+    Wb[k, i, j] = value
+    y, y0 = run_conv(h, c, X, Wb, 2, use_h), run_conv(h, c, X, W0, 2, use_h)
+    ref_bad, bad = ~torch.isfinite(sn.conv64(c[3], X, Wb)), ~torch.isfinite(y)
+    assert ref_bad.any()
+    assert bad[ref_bad].all(), "an output that reads the non-finite weight is finite"
+    others = torch.ones_like(bad)
+    others[:, j] = False
+    assert not bad[others].any(), "a non-finite output outside the weight's channel"
+    assert sn.same_bits(y[others], y0[others]), "an output of another channel changed"
