@@ -392,6 +392,23 @@ int lb2_pc_nn(void* h, void* stream, const double* q, int32_t nq, const void* tr
 int lb2_segment_sum(void* h, void* stream, const void* values, int32_t f64, const int64_t* order, const int64_t* offsets,
                     int64_t nseg, int32_t c, void* out);
 
+/* Deterministic segmented product-sum under skewed segment lengths (the gradient of the conditioning gates' gather x * table[idx]):
+ *     out[s][j] = sum over i in [offsets[s], offsets[s + 1]) of a[order[i]][j] * b[order[i]][j]        (b == NULL: of a[order[i]][j])
+ * a, b (rows, c) fp32, 1 <= c <= 256 (others: LB2_ERR_ARG); order int64[nrows] (NULL = identity); offsets int64[nseg + 1],
+ * non-decreasing with offsets[0] = 0 and offsets[nseg] = nrows; out (nseg, c) fp32; scratch >= lb2_segment_dot_scratch_bytes(nrows, c).
+ * nseg == 0 writes nothing; nrows == 0 writes zeros.  The work is split by position, not by segment, so one segment that holds
+ * every row costs what many short ones do.  Summation order, per channel j, with R = LB2_SEGMENT_DOT_R, every product one
+ * round-to-nearest multiply and every addition one round-to-nearest add (no FMA):
+ *   - chunk k is the positions [k R, min((k + 1) R, nrows)); the pieces of segment s are its non-empty intersections with the chunks;
+ *   - a piece's sum starts from +0 and adds its products in ascending position i;
+ *   - a segment with one piece is that piece's sum; a segment with several is +0 plus its pieces' sums in ascending chunk order; a
+ *     segment without rows is +0.
+ * So the result depends on the inputs only (no atomics), and a NaN or inf in a row reaches its own segment's sum and no other. */
+#define LB2_SEGMENT_DOT_R 128
+size_t lb2_segment_dot_scratch_bytes(int64_t nrows, int32_t c);
+int lb2_segment_dot(void* h, void* stream, const float* a, const float* b, const int64_t* order, const int64_t* offsets,
+                    int64_t nrows, int64_t nseg, int32_t c, float* out, void* scratch);
+
 /* Point normals as open3d 0.17's PointCloud.estimate_normals() computes them (KDTreeSearchParamKNN(30), fast_normal_computation;
  * tools/diff_completion_pipeline.py:204-212), in two steps over a tree from lb2_pc_tree_build(pts, n):
  *   lb2_pc_knn      exact self-k-nearest neighbours, 1 <= k <= 32 (larger k: LB2_ERR_UNSUP).  With k_eff = min(k, n), row j of

@@ -74,6 +74,7 @@ EXPORTS = [
     "lb2_aggregate_window_scratch_bytes", "lb2_aggregate_window", "lb2_jitter_filter_scratch_bytes", "lb2_jitter_filter",
     "lb2_voxel_first_f64_scratch_bytes", "lb2_voxel_first_f64",
     "lb2_spconv_wgrad_scratch_bytes", "lb2_spconv_wgrad", "lb2_segment_sum",
+    "lb2_segment_dot_scratch_bytes", "lb2_segment_dot",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -195,6 +196,9 @@ class Lib:
         d.lb2_spconv_wgrad_scratch_bytes.restype = C.c_size_t
         d.lb2_spconv_wgrad.argtypes = [vp, vp, vp, i32, vp, i32, i32, vp, i64, i32, vp, vp]
         d.lb2_segment_sum.argtypes = [vp, vp, vp, i32, vp, vp, i64, i32, vp]
+        d.lb2_segment_dot_scratch_bytes.argtypes = [i64, i32]
+        d.lb2_segment_dot_scratch_bytes.restype = C.c_size_t
+        d.lb2_segment_dot.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, i32, vp, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -334,6 +338,16 @@ class Handle:
         """out[s] = sum of values[order[i]] over i in [offsets[s], offsets[s + 1]), in ascending i (order None: identity)"""
         self._check(self.dll.lb2_segment_sum(self.hp, self._stream(), _ptr(values), int(values.dtype == torch.float64), _ptr(order),
                                              _ptr(offsets), int(offsets.shape[0] - 1), int(values.shape[1]), _ptr(out)), "lb2_segment_sum")
+
+    def segment_dot(self, a, b, order, offsets, out):
+        """out[s] = sum of a[order[i]] * b[order[i]] over i in [offsets[s], offsets[s + 1]) in lb2_segment_dot's chunked order (b None:
+        of a[order[i]]); a, b (rows, c) fp32, order int64 over every row"""
+        if a.dtype != torch.float32 or (b is not None and b.dtype != torch.float32):
+            raise RuntimeError("lb2_segment_dot: fp32 operands only")
+        nrows, c = (a.shape[0] if order is None else order.shape[0]), a.shape[1]
+        scratch = torch.empty(int(self.dll.lb2_segment_dot_scratch_bytes(int(nrows), int(c))), dtype=torch.uint8, device=self.device)
+        self._check(self.dll.lb2_segment_dot(self.hp, self._stream(), _ptr(a), _ptr(b), _ptr(order), _ptr(offsets), int(nrows),
+                                             int(offsets.shape[0] - 1), int(c), _ptr(out), _ptr(scratch)), "lb2_segment_dot")
 
     # -- misc ----------------------------------------------------------------------------------------
     def nn_match(self, q, d_nq, nq_cap, k, d_nk, nk_cap, batch_scale, idx):

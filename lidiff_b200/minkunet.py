@@ -13,6 +13,7 @@ import torch
 import torch.nn as nn
 
 from . import me as ME
+from .gate import GateMul, TakeRows
 from .keops import LazyTensor
 
 __all__ = ["MinkGlobalEnc", "MinkUNetDiff", "MinkUNet"]
@@ -150,23 +151,45 @@ class MinkUNetDiff(_Backbone):
             emb = nn.functional.pad(emb, (0, 1), "constant", 0)
         return emb
 
-    def match_part_to_full(self, x_full, x_part):
+    def _match_index(self, x_full, x_part):
+        """row of x_part nearest to every row of x_full, within the row's batch"""
         full_c = x_full.C.clone().float()
         part_c = x_part.C.clone().float()
         scale = full_c.max() * 2.0                       # "hash" the batch coordinate apart
         full_c[:, 0] *= scale
         part_c[:, 0] *= scale
         d = ((LazyTensor(full_c[:, None, :]) - LazyTensor(part_c[None, :, :])) ** 2).sum(-1)
-        return x_part.F[d.argKmin(1, dim=1)[:, 0]]
+        return d.argKmin(1, dim=1)[:, 0]
+
+    def match_part_to_full(self, x_full, x_part):
+        return x_part.F[self._match_index(x_full, x_part)]
+
+    def _gate_hoisted(self, name, x, part_feats, temp_emb):
+        """the gate with gradients.  The three MLPs act row by row and a voxel row's inputs are those of its part voxel and its
+        batch, so they run once per part row and every voxel row gathers its result (GateMul): the same expression as _gate's,
+        without saving the MLPs' activations per voxel row."""
+        part_batch = part_feats.C[:, 0].long()
+        absent = torch.nonzero(torch.bincount(part_batch, minlength=temp_emb.shape[0])[: temp_emb.shape[0]] == 0)[:, 0].tolist()
+        if absent:
+            raise ValueError(f"MinkUNetDiff: no part voxel in batch {absent}: a voxel of that batch would take another scan's condition")
+        p = getattr(self, f"latent_{name}")(part_feats.F)
+        t = TakeRows.apply(getattr(self, f"{name}_temp")(temp_emb), part_batch)
+        pair = (t, p) if name == "up1" else (p, t)
+        table = getattr(self, f"latemp_{name}")(torch.cat(pair, -1))
+        return x._like(GateMul.apply(x.F, table, self._match_index(x, part_feats)))
 
     def _gate(self, g, x, part_feats, temp_emb):
         name = self._GATES[g]
-        p = getattr(self, f"latent_{name}")(self.match_part_to_full(x, part_feats))
-        t = getattr(self, f"{name}_temp")(temp_emb)
+        mlps = [getattr(self, f"latent_{name}"), getattr(self, f"{name}_temp"), getattr(self, f"latemp_{name}")]
+        if torch.is_grad_enabled() and (x.F.requires_grad or part_feats.F.requires_grad or temp_emb.requires_grad
+                                        or any(w.requires_grad for m in mlps for w in m.parameters())):
+            return self._gate_hoisted(name, x, part_feats, temp_emb)
+        p = mlps[0](self.match_part_to_full(x, part_feats))
+        t = mlps[1](temp_emb)
         per_batch = torch.unique(x.C[:, 0], return_counts=True)[1]
         t = torch.repeat_interleave(t, per_batch, dim=0)
         pair = (t, p) if name == "up1" else (p, t)       # the reference concatenates (t4, p4) for up1 only
-        return x * getattr(self, f"latemp_{name}")(torch.cat(pair, -1))
+        return x * mlps[2](torch.cat(pair, -1))
 
     def forward(self, x, x_sparse, part_feats, t):
         temp_emb = self.get_timestep_embedding(t)
