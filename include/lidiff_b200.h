@@ -409,6 +409,57 @@ size_t lb2_segment_dot_scratch_bytes(int64_t nrows, int32_t c);
 int lb2_segment_dot(void* h, void* stream, const float* a, const float* b, const int64_t* order, const int64_t* offsets,
                     int64_t nrows, int64_t nseg, int32_t c, float* out, void* scratch);
 
+/* Synchronised batch norm (training mode over the rows of every rank; lidiff_b200.me.MinkowskiSyncBatchNorm).  Each rank passes its
+ * own rows x (n, c) fp32, 0 <= n < 2^31, 1 <= c <= 1024; the caller combines the int64 word arrays across ranks between the calls
+ * (MAX for *max_words, SUM for *sum_words / sq_words) and the global row count N = sum of n must stay below 2^31 (a combined
+ * count outside 1 <= N < 2^31 makes mean, var, invstd, y, dx and the running statistics NaN, as the words may have wrapped).  Every output
+ * depends only on the multiset of rows: not on their order, the launch or the split across ranks.  Per channel j, with
+ * RN64 / RN32 one round-to-nearest-even fp64 / fp32 operation each (no FMA), e(v) the exponent with v < 2^e(v) (e(0) = 0) and
+ * RNI(v) the nearest integer (ties to even):
+ *
+ *   lb2_sync_bn_max      max_words[2j] = bits of M = the largest finite |x|, max_words[2j+1] = 1 if x holds a NaN or +-inf.  [MAX]
+ *   lb2_sync_bn_sum      q = RNI(x 2^s), s = 62 - e(M), |q| <= 2^62; sum_words[2j] = sum (q >> 32), sum_words[2j+1] = sum (q & (2^32 - 1)),
+ *                        sum_words[2c] = n.  S = sum_words[2j] 2^32 + sum_words[2j+1] is exact.                              [SUM]
+ *   lb2_sync_bn_sumsq    mean[j] = mu = RN64(S / N) 2^-s (the quotient of the integers rounded once); then d = RN64(x - mu),
+ *                        p = RNI(d 2^t), t = 62 - e(RN64(M + |mu|)), and sq_words[4j + k] = the sum of 32-bit limb k of p^2 (< 2^125).
+ *                        T = sum_k sq_words[4j + k] 2^(32 k) is exact.                                                       [SUM]
+ *   lb2_sync_bn_apply    var[j] = RN64(T / N) 2^-2t (biased, as torch normalises), invstd[j] = RN64(1 / RN64(sqrt(RN64(var + eps)))),
+ *                        y = RN32(RN64(RN64(RN64(d invstd) gamma) + beta)) (gamma / beta NULL: 1 / 0);
+ *                        with running statistics (a = momentum): rm = RN32(RN64(RN64((1 - a) rm) + RN64(a mu))),
+ *                        rv = RN32(RN64(RN64((1 - a) rv) + RN64(a u))), u = RN64(RN64(var N) / (N - 1)) (N = 1: NaN).
+ * A flagged channel (max_words[2j+1]) has mu = var = invstd = NaN and y[:, j] = NaN on every rank; the other channels keep their bits.
+ *
+ * Words: |q|, |p| <= 2^62 give 32-bit limbs, and N < 2^31 rows keep every word's sum below 2^63 on one rank and after the SUM across
+ * ranks.  Error against exact arithmetic (m, v the exact mean and biased variance of the union, B = M + |mu| <= 2M (1 + 2^-52)):
+ *   |mu - m|   <= 2^-62 M + 2^-53 |m|
+ *   |var - v|  <= 2^-50 v + 2^-59 B sqrt(v) + 2^-100 B^2
+ * (each q and p is within 1/2 of its scaled value, d carries one fp64 rounding, the quotients one each).  For v >= 2^-40 M^2 the
+ * relative error of var is below 2^-37, far below fp32's 2^-24.
+ *
+ * Backward, with xhat = RN64(d invstd) and g = RN64(dy xhat) in the forward's formulas:
+ *   lb2_sync_bn_backward_max   max_words[3j] = bits of the largest finite |dy| (fp32), [3j+1] = bits of the largest finite |g| (fp64),
+ *                              [3j+2] = 1 if a dy or g is NaN or +-inf.                                                      [MAX]
+ *   lb2_sync_bn_backward_sum   a = RNI(dy 2^sa), sa = 62 - e(max|dy|); b = RNI(g 2^sb), sb = 62 - e(max|g|); sum_words[4j .. 4j+3] =
+ *                              the hi / lo words of sum a and of sum b as above.  This rank's parameter gradients (NULL: skipped)
+ *                              dbeta = RN32(RN64(A) 2^-sa), dgamma = RN32(RN64(Bs) 2^-sb) from these local words.            [SUM]
+ *   lb2_sync_bn_backward_apply mdy = RN64(A / N) 2^-sa, mg = RN64(Bs / N) 2^-sb from the combined words, N = *count (the forward's
+ *                              sum_words[2c]); dx = RN32(RN64(k RN64(RN64(dy - mdy) - RN64(xhat mg)))), k = RN64(gamma invstd).
+ * A flagged channel has dx[:, j], dgamma[j], dbeta[j] = NaN.  No float atomics. */
+int lb2_sync_bn_max(void* h, void* stream, const float* x, int64_t n, int32_t c, int64_t* max_words);
+int lb2_sync_bn_sum(void* h, void* stream, const float* x, int64_t n, int32_t c, const int64_t* max_words, int64_t* sum_words);
+int lb2_sync_bn_sumsq(void* h, void* stream, const float* x, int64_t n, int32_t c, const int64_t* max_words, const int64_t* sum_words,
+                      double* mean, int64_t* sq_words);
+int lb2_sync_bn_apply(void* h, void* stream, const float* x, int64_t n, int32_t c, const int64_t* max_words, const int64_t* sum_words,
+                      const double* mean, const int64_t* sq_words, const float* gamma, const float* beta, double eps, double momentum,
+                      float* running_mean, float* running_var, double* var, double* invstd, float* y);
+int lb2_sync_bn_backward_max(void* h, void* stream, const float* dy, const float* x, int64_t n, int32_t c, const double* mean,
+                             const double* invstd, int64_t* max_words);
+int lb2_sync_bn_backward_sum(void* h, void* stream, const float* dy, const float* x, int64_t n, int32_t c, const double* mean,
+                             const double* invstd, const int64_t* max_words, int64_t* sum_words, float* dgamma, float* dbeta);
+int lb2_sync_bn_backward_apply(void* h, void* stream, const float* dy, const float* x, int64_t n, int32_t c, const double* mean,
+                               const double* invstd, const float* gamma, const int64_t* max_words, const int64_t* sum_words,
+                               const int64_t* count, float* dx);
+
 /* Point normals as open3d 0.17's PointCloud.estimate_normals() computes them (KDTreeSearchParamKNN(30), fast_normal_computation;
  * tools/diff_completion_pipeline.py:204-212), in two steps over a tree from lb2_pc_tree_build(pts, n):
  *   lb2_pc_knn      exact self-k-nearest neighbours, 1 <= k <= 32 (larger k: LB2_ERR_UNSUP).  With k_eff = min(k, n), row j of

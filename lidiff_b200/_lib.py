@@ -75,6 +75,8 @@ EXPORTS = [
     "lb2_voxel_first_f64_scratch_bytes", "lb2_voxel_first_f64",
     "lb2_spconv_wgrad_scratch_bytes", "lb2_spconv_wgrad", "lb2_segment_sum",
     "lb2_segment_dot_scratch_bytes", "lb2_segment_dot",
+    "lb2_sync_bn_max", "lb2_sync_bn_sum", "lb2_sync_bn_sumsq", "lb2_sync_bn_apply",
+    "lb2_sync_bn_backward_max", "lb2_sync_bn_backward_sum", "lb2_sync_bn_backward_apply",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -199,6 +201,13 @@ class Lib:
         d.lb2_segment_dot_scratch_bytes.argtypes = [i64, i32]
         d.lb2_segment_dot_scratch_bytes.restype = C.c_size_t
         d.lb2_segment_dot.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, i32, vp, vp]
+        d.lb2_sync_bn_max.argtypes = [vp, vp, vp, i64, i32, vp]
+        d.lb2_sync_bn_sum.argtypes = [vp, vp, vp, i64, i32, vp, vp]
+        d.lb2_sync_bn_sumsq.argtypes = [vp, vp, vp, i64, i32, vp, vp, vp, vp]
+        d.lb2_sync_bn_apply.argtypes = [vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, f64, f64, vp, vp, vp, vp, vp]
+        d.lb2_sync_bn_backward_max.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp]
+        d.lb2_sync_bn_backward_sum.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp]
+        d.lb2_sync_bn_backward_apply.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -348,6 +357,52 @@ class Handle:
         scratch = torch.empty(int(self.dll.lb2_segment_dot_scratch_bytes(int(nrows), int(c))), dtype=torch.uint8, device=self.device)
         self._check(self.dll.lb2_segment_dot(self.hp, self._stream(), _ptr(a), _ptr(b), _ptr(order), _ptr(offsets), int(nrows),
                                              int(offsets.shape[0] - 1), int(c), _ptr(out), _ptr(scratch)), "lb2_segment_dot")
+
+    # -- synchronised batch norm (include/lidiff_b200.h: the words, formulas and the collective between each call) ---------------
+    def sync_bn_max(self, x, max_words):
+        """max_words int64 (2c,): per channel the largest finite |x| (fp32 bits) and a non-finite flag; combine with MAX"""
+        n, c = x.shape
+        self._check(self.dll.lb2_sync_bn_max(self.hp, self._stream(), _ptr(x), int(n), int(c), _ptr(max_words)), "lb2_sync_bn_max")
+
+    def sync_bn_sum(self, x, max_words, sum_words):
+        """sum_words int64 (2c + 1,): the fixed-point sum of x per channel and the row count; combine with SUM"""
+        n, c = x.shape
+        self._check(self.dll.lb2_sync_bn_sum(self.hp, self._stream(), _ptr(x), int(n), int(c), _ptr(max_words), _ptr(sum_words)),
+                    "lb2_sync_bn_sum")
+
+    def sync_bn_sumsq(self, x, max_words, sum_words, mean, sq_words):
+        """mean fp64 (c,) from the combined sums; sq_words int64 (4c,): the fixed-point sum of (x - mean)^2; combine with SUM"""
+        n, c = x.shape
+        self._check(self.dll.lb2_sync_bn_sumsq(self.hp, self._stream(), _ptr(x), int(n), int(c), _ptr(max_words), _ptr(sum_words),
+                                               _ptr(mean), _ptr(sq_words)), "lb2_sync_bn_sumsq")
+
+    def sync_bn_apply(self, x, max_words, sum_words, mean, sq_words, gamma, beta, eps, momentum, running_mean, running_var, var, invstd,
+                      y):
+        """var, invstd fp64 (c,), the running statistics (None: not tracked) and y = the normalised x"""
+        n, c = x.shape
+        self._check(self.dll.lb2_sync_bn_apply(self.hp, self._stream(), _ptr(x), int(n), int(c), _ptr(max_words), _ptr(sum_words), _ptr(mean),
+                                               _ptr(sq_words), _ptr(gamma), _ptr(beta), float(eps), float(momentum), _ptr(running_mean),
+                                               _ptr(running_var), _ptr(var), _ptr(invstd), _ptr(y)), "lb2_sync_bn_apply")
+
+    def sync_bn_backward_max(self, dy, x, mean, invstd, max_words):
+        """max_words int64 (3c,): the largest finite |dy| and |dy xhat| and a non-finite flag per channel; combine with MAX"""
+        n, c = x.shape
+        self._check(self.dll.lb2_sync_bn_backward_max(self.hp, self._stream(), _ptr(dy), _ptr(x), int(n), int(c), _ptr(mean), _ptr(invstd),
+                                                      _ptr(max_words)), "lb2_sync_bn_backward_max")
+
+    def sync_bn_backward_sum(self, dy, x, mean, invstd, max_words, sum_words, dgamma, dbeta):
+        """sum_words int64 (4c,): the fixed-point sums of dy and dy xhat (combine with SUM); dgamma / dbeta: this rank's sums"""
+        n, c = x.shape
+        self._check(self.dll.lb2_sync_bn_backward_sum(self.hp, self._stream(), _ptr(dy), _ptr(x), int(n), int(c), _ptr(mean), _ptr(invstd),
+                                                      _ptr(max_words), _ptr(sum_words), _ptr(dgamma), _ptr(dbeta)),
+                    "lb2_sync_bn_backward_sum")
+
+    def sync_bn_backward_apply(self, dy, x, mean, invstd, gamma, max_words, sum_words, count, dx):
+        """dx from the combined backward sums; count = the forward's combined sum_words[2c:]"""
+        n, c = x.shape
+        self._check(self.dll.lb2_sync_bn_backward_apply(self.hp, self._stream(), _ptr(dy), _ptr(x), int(n), int(c), _ptr(mean), _ptr(invstd),
+                                                        _ptr(gamma), _ptr(max_words), _ptr(sum_words), _ptr(count), _ptr(dx)),
+                    "lb2_sync_bn_backward_apply")
 
     # -- misc ----------------------------------------------------------------------------------------
     def nn_match(self, q, d_nq, nq_cap, k, d_nk, nk_cap, batch_scale, idx):

@@ -463,10 +463,119 @@ class MinkowskiBatchNorm(nn.Module):
         return x._like(self.bn(x.F))
 
 
+_SYNC_GROUPS = {}
+
+
+def _sync_group(process_group):
+    """the process group the sync-BN collectives run on: the given one, or else one of their own over every rank, created once per
+    default group (all ranks reach their first sync-BN forward together, so they create it in the same order).  On a group of
+    their own the layers' collectives cannot interleave differently from DDP's gradient all-reduces on different ranks."""
+    import torch.distributed as dist
+    if process_group is not None:
+        return process_group
+    world = dist.group.WORLD
+    got = _SYNC_GROUPS.get(id(world))
+    if got is None or got[0] is not world:
+        got = (world, dist.new_group(ranks=list(range(dist.get_world_size()))))
+        _SYNC_GROUPS[id(world)] = got
+    return got[1]
+
+
+class _SyncBatchNormFn(torch.autograd.Function):
+    """training-mode batch norm over the rows of every rank of `group` (lb2_sync_bn_*: three collectives forward, two backward, on
+    the current stream).  The parameter gradients are this rank's sums, as torch's SyncBatchNorm returns them; DDP averages them."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, bn, group, factor):
+        import torch.distributed as dist
+        h = _lib.get_handle(x.device)
+        n, c = x.shape
+        i64 = dict(dtype=torch.int64, device=x.device)
+        mw = torch.empty(2 * c, **i64)
+        h.sync_bn_max(x, mw)
+        dist.all_reduce(mw, dist.ReduceOp.MAX, group=group)
+        sw = torch.empty(2 * c + 1, **i64)
+        h.sync_bn_sum(x, mw, sw)
+        dist.all_reduce(sw, group=group)
+        mean = torch.empty(c, dtype=torch.float64, device=x.device)
+        qw = torch.empty(4 * c, **i64)
+        h.sync_bn_sumsq(x, mw, sw, mean, qw)
+        dist.all_reduce(qw, group=group)
+        var, invstd, y = torch.empty_like(mean), torch.empty_like(mean), torch.empty_like(x)
+        track = bn.track_running_stats and bn.running_mean is not None
+        h.sync_bn_apply(x, mw, sw, mean, qw, weight, bias, bn.eps, factor, bn.running_mean if track else None,
+                        bn.running_var if track else None, var, invstd, y)
+        ctx.save_for_backward(x, weight, mean, invstd, sw)
+        ctx.group = group
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        import torch.distributed as dist
+        x, weight, mean, invstd, sw = ctx.saved_tensors
+        h = _lib.get_handle(x.device)
+        dy = dy.contiguous()
+        c = x.shape[1]
+        mw = torch.empty(3 * c, dtype=torch.int64, device=x.device)
+        h.sync_bn_backward_max(dy, x, mean, invstd, mw)
+        dist.all_reduce(mw, dist.ReduceOp.MAX, group=ctx.group)
+        bw = torch.empty(4 * c, dtype=torch.int64, device=x.device)
+        dgamma = torch.empty(c, dtype=torch.float32, device=x.device) if ctx.needs_input_grad[1] else None
+        dbeta = torch.empty(c, dtype=torch.float32, device=x.device) if ctx.needs_input_grad[2] else None
+        h.sync_bn_backward_sum(dy, x, mean, invstd, mw, bw, dgamma, dbeta)
+        dist.all_reduce(bw, group=ctx.group)
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            h.sync_bn_backward_apply(dy, x, mean, invstd, weight, mw, bw, sw[2 * c:], dx)
+        return dx, dgamma, dbeta, None, None, None
+
+
 class MinkowskiSyncBatchNorm(MinkowskiBatchNorm):
+    """ME.MinkowskiSyncBatchNorm: the same `.bn` (parameters, buffers, state-dict keys) as MinkowskiBatchNorm.  In training mode
+    with a process group of more than one rank the statistics are those of every rank's rows (lb2_sync_bn_*: every output depends
+    only on the multiset of rows, whatever their split across ranks); otherwise it is exactly MinkowskiBatchNorm, as torch's
+    SyncBatchNorm falls back to BatchNorm."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True, process_group=None):
+        super().__init__(num_features, eps=eps, momentum=momentum, affine=affine, track_running_stats=track_running_stats)
+        self.process_group = process_group
+
+    def _world(self):
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized()):
+            return 1
+        return dist.get_world_size(self.process_group)
+
+    def forward(self, x: SparseTensor) -> SparseTensor:
+        if not self.training or self._world() < 2:
+            return super().forward(x)
+        bn = self.bn
+        # the momentum and num_batches_tracked bookkeeping of nn.BatchNorm1d.forward
+        factor = 0.0 if bn.momentum is None else bn.momentum
+        if bn.track_running_stats and bn.num_batches_tracked is not None:
+            bn.num_batches_tracked.add_(1)
+            factor = 1.0 / float(bn.num_batches_tracked) if bn.momentum is None else bn.momentum
+        F = x.F
+        if F.dim() != 2 or F.dtype != torch.float32 or F.shape[1] != bn.num_features:
+            raise RuntimeError(f"MinkowskiSyncBatchNorm({bn.num_features}): features must be (rows, {bn.num_features}) fp32")
+        y = _SyncBatchNormFn.apply(F.contiguous(), bn.weight, bn.bias, bn, _sync_group(self.process_group), factor)
+        return x._like(y)
+
     @classmethod
     def convert_sync_batchnorm(cls, module, process_group=None):
-        return module          # single-process inference path; training-side sync BN is out of scope (SURVEY.md 8f-3)
+        """every MinkowskiBatchNorm in `module` replaced by a MinkowskiSyncBatchNorm holding the same `.bn` (so the same parameters,
+        buffers and state-dict keys); returns the converted module, as torch.nn.SyncBatchNorm.convert_sync_batchnorm does"""
+        out = module
+        if isinstance(module, MinkowskiBatchNorm) and not isinstance(module, MinkowskiSyncBatchNorm):
+            b = module.bn
+            out = cls(b.num_features, eps=b.eps, momentum=b.momentum, affine=b.affine, track_running_stats=b.track_running_stats,
+                      process_group=process_group)
+            out.bn = b
+            out.train(module.training)
+        for name, child in module.named_children():
+            out.add_module(name, cls.convert_sync_batchnorm(child, process_group))
+        return out
 
 
 class MinkowskiReLU(nn.Module):

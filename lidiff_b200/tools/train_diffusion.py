@@ -13,9 +13,14 @@ filter, as tools/test_completion scores it: Chamfer mean / std, precision / reca
 state_dict (partial_enc.*, model.*), optimizer_states, lr_schedulers, epoch, global_step, hyper_parameters.
 
 --max-steps N (not in the reference) stops this run after N optimiser steps and writes the checkpoint of the epoch it stopped in.
-DistributedDataParallel, SyncBatchNorm, TensorBoard and the open3d viewer are not built: training is single-GPU.
+
+Under torchrun every rank trains on its own shard (lidiff_b200.ddp): synchronised batch norm, DistributedDataParallel averaging the
+gradients, no learning-rate scaling, `train.n_gpus` = the world size in hyper_parameters.  Rank 0 prints the mean over ranks of the
+logged scalars and of the validation scores (each rank completes the first batch of its own validation shard) and writes the
+checkpoint, which loads unchanged in a single process.  TensorBoard and the open3d viewer are not built.
 
     python -m lidiff_b200.tools.train_diffusion -c lidiff/config/config.yaml
+    torchrun --nproc-per-node 8 -m lidiff_b200.tools.train_diffusion -c lidiff/config/config.yaml
     python -m lidiff_b200.tools.train_diffusion -c config.yaml -ckpt experiments/prob10_5p0reg/checkpoints/prob10_5p0reg_epoch=04.ckpt
 """
 from __future__ import annotations
@@ -28,6 +33,7 @@ import torch
 import torch.nn as nn
 import yaml
 
+from .. import ddp
 from .. import me as ME
 from ..datasets import TemporalKittiDataModule
 from ..minkunet import MinkGlobalEnc, MinkUNetDiff
@@ -162,13 +168,16 @@ def load_checkpoint(path, nets, opt=None, sched=None):
 @click.option("--max-steps", type=int, default=None, help="stop this run after this many optimiser steps")
 def main(config, weights, checkpoint, out, max_steps):
     set_deterministic()
+    run = ddp.start()
     with open(config) as f:
         cfg = yaml.safe_load(f)
     if os.environ.get("TRAIN_DATABASE"):
         cfg["data"]["data_dir"] = os.environ["TRAIN_DATABASE"]
     cfg["data"].setdefault("dataset_norm", False)
     cfg["data"].setdefault("std_axis_norm", False)
-    device = torch.device("cuda", torch.cuda.current_device())
+    if run.distributed:
+        cfg["train"]["n_gpus"] = run.world
+    device = run.device
     out = out or os.path.join("experiments", cfg["experiment"]["id"], "checkpoints")
     os.makedirs(out, exist_ok=True)
     somac = sqrt_one_minus_alphas_cumprod(cfg)
@@ -180,28 +189,40 @@ def main(config, weights, checkpoint, out, max_steps):
         first_epoch, step = int(ckpt["epoch"]) + 1, int(ckpt["global_step"])
     elif weights is not None:
         load_checkpoint(weights, nets)
-    nets.train()
-    print("TRAINING MODE")
+    model, nets = ddp.wrap(nets, run)
+    model.train()
+    if run.main:
+        print("TRAINING MODE")
     dm = TemporalKittiDataModule(cfg, device=device)
-    train_loader, val_loader = dm.train_dataloader(), dm.val_dataloader()
+    train_loader = ddp.sharded(dm.train_dataloader(), run, shuffle=True)
+    val_loader = ddp.sharded(dm.val_dataloader(), run, shuffle=False)
     last_step = None if max_steps is None else step + max_steps
     for epoch in range(first_epoch, int(cfg["train"]["max_epoch"])):
+        ddp.set_epoch(train_loader, epoch)
+        ddp.set_epoch(val_loader, epoch)
         for batch in train_loader:
-            log = train_step(nets, opt, batch, cfg, somac, device)
-            print(f"epoch {epoch} step {step}" + ("" if not log["uncond"] else " (unconditional)") + " "
-                  + " ".join(f"train/{k}: {log[k].item():.9g}" for k in LOGGED))
+            log = train_step(model, opt, batch, cfg, somac, device)
+            means = ddp.mean_over_ranks([log[k] for k in LOGGED], run, device)
+            if run.main:
+                print(f"epoch {epoch} step {step}" + ("" if not log["uncond"] else " (unconditional)") + " "
+                      + " ".join(f"train/{k}: {v:.9g}" for k, v in zip(LOGGED, means)))
             step += 1
             if step == last_step:
                 break
         end_epoch(sched, epoch)
         if (epoch + 1) % VAL_EVERY == 0 and step != last_step:
-            val = validate(nets, next(iter(val_loader)), cfg, device)
-            print(f"epoch {epoch} " + " ".join(f"val/{k}: {v:.9g}" for k, v in zip(("cd_mean", "cd_std", "precision", "recall", "fscore"), val)))
+            val = ddp.mean_over_ranks(validate(nets, next(iter(val_loader)), cfg, device), run, device)
+            if run.main:
+                print(f"epoch {epoch} " + " ".join(f"val/{k}: {v:.9g}" for k, v in zip(("cd_mean", "cd_std", "precision", "recall", "fscore"), val)))
         path = checkpoint_path(out, cfg, epoch)
-        save_checkpoint(path, nets, opt, sched, cfg, epoch, step)
-        print(f"saved {path}")
+        if run.distributed:
+            torch.distributed.barrier()
+        if run.main:
+            save_checkpoint(path, nets, opt, sched, cfg, epoch, step)
+            print(f"saved {path}")
         if step == last_step:
             break
+    ddp.finish(run)
 
 
 if __name__ == "__main__":

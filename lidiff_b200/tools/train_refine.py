@@ -8,8 +8,15 @@ CUDA gradients (lidiff_b200.me) and one Adam step (lr = train.lr, betas (0.9, 0.
 the mean over the first 5 % of the validation batches, as the reference's Trainer (check_val_every_n_epoch=5,
 limit_val_batches=0.05).  After every epoch <out>/<experiment.id>_epoch=NN.ckpt holds the Lightning checkpoint fields the
 reference and tools/test_refine read: state_dict (model_refine.*), optimizer_states, epoch, global_step, hyper_parameters.
+--max-steps N (not in the reference) stops this run after N optimiser steps and writes the checkpoint of the epoch it stopped in.
+
+Under torchrun every rank trains on its own shard (lidiff_b200.ddp): synchronised batch norm, DistributedDataParallel averaging the
+gradients, no learning-rate scaling, `train.n_gpus` = the world size in hyper_parameters.  Rank 0 prints the mean over ranks of the
+loss and of val/cd_loss (each rank takes the first 5 % of its own validation shard's batches, at least one) and writes the
+checkpoint, which loads unchanged in a single process.
 
     python -m lidiff_b200.tools.train_refine -c lidiff/config/config_refine.yaml
+    torchrun --nproc-per-node 8 -m lidiff_b200.tools.train_refine -c lidiff/config/config_refine.yaml
     python -m lidiff_b200.tools.train_refine -c config_refine.yaml -ckpt experiments/Refine_Up6/checkpoints/Refine_Up6_epoch=02.ckpt
 """
 from __future__ import annotations
@@ -20,6 +27,7 @@ import click
 import torch
 import yaml
 
+from .. import ddp
 from ..datasets_refine import TemporalKittiDataModule
 from ..minkunet import MinkUNet
 from .test_completion import set_deterministic
@@ -86,13 +94,17 @@ def load_checkpoint(path, net, opt=None):
 @click.option("--weights", "-w", type=str, default=None, help="start from these weights (.ckpt) without resuming training")
 @click.option("--checkpoint", "-ckpt", type=str, default=None, help="resume training from this checkpoint (.ckpt)")
 @click.option("--out", type=str, default=None, help="checkpoint directory (default experiments/<experiment.id>/checkpoints)")
-def main(config, weights, checkpoint, out):
+@click.option("--max-steps", type=int, default=None, help="stop this run after this many optimiser steps")
+def main(config, weights, checkpoint, out, max_steps):
     set_deterministic()
+    run = ddp.start()
     with open(config) as f:
         cfg = yaml.safe_load(f)
     if os.environ.get("TRAIN_DATABASE"):
         cfg["data"]["data_dir"] = os.environ["TRAIN_DATABASE"]
-    device = torch.device("cuda", torch.cuda.current_device())
+    if run.distributed:
+        cfg["train"]["n_gpus"] = run.world
+    device = run.device
     out = out or os.path.join("experiments", cfg["experiment"]["id"], "checkpoints")
     os.makedirs(out, exist_ok=True)
     net = MinkUNet(in_channels=3, out_channels=3 * int(cfg["train"]["up_factor"])).to(device)
@@ -103,19 +115,35 @@ def main(config, weights, checkpoint, out):
         first_epoch, step = int(ckpt["epoch"]) + 1, int(ckpt["global_step"])
     elif weights is not None:
         load_checkpoint(weights, net)
-    net.train()
+    model, net = ddp.wrap(net, run)
+    model.train()
     dm = TemporalKittiDataModule(cfg, device=device)
-    train_loader, val_loader = dm.train_dataloader(), dm.val_dataloader()
+    train_loader = ddp.sharded(dm.train_dataloader(), run, shuffle=True)
+    val_loader = ddp.sharded(dm.val_dataloader(), run, shuffle=False)
+    last_step = None if max_steps is None else step + max_steps
     for epoch in range(first_epoch, int(cfg["train"]["max_epoch"])):
+        ddp.set_epoch(train_loader, epoch)
+        ddp.set_epoch(val_loader, epoch)
         for batch in train_loader:
-            loss = train_step(net, opt, batch, cfg, device)
-            print(f"epoch {epoch} step {step} train/cd_loss: {loss.item():.9g}")
+            loss = ddp.mean_over_ranks([train_step(model, opt, batch, cfg, device)], run, device)[0]
+            if run.main:
+                print(f"epoch {epoch} step {step} train/cd_loss: {loss:.9g}")
             step += 1
-        if (epoch + 1) % VAL_EVERY == 0:
-            print(f"epoch {epoch} val/cd_loss: {validate(net, val_loader, cfg, device):.9g}")
+            if step == last_step:
+                break
+        if (epoch + 1) % VAL_EVERY == 0 and step != last_step:
+            val = ddp.mean_over_ranks([validate(net, val_loader, cfg, device)], run, device)[0]
+            if run.main:
+                print(f"epoch {epoch} val/cd_loss: {val:.9g}")
         path = checkpoint_path(out, cfg, epoch)
-        save_checkpoint(path, net, opt, cfg, epoch, step)
-        print(f"saved {path}")
+        if run.distributed:
+            torch.distributed.barrier()
+        if run.main:
+            save_checkpoint(path, net, opt, cfg, epoch, step)
+            print(f"saved {path}")
+        if step == last_step:
+            break
+    ddp.finish(run)
 
 
 if __name__ == "__main__":
