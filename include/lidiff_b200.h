@@ -312,7 +312,7 @@ int lb2_nn_match_tree(void* h, void* stream, const int32_t* q_coords, const int3
 
 /* ---- small dense layers — torch.nn.Linear (+LeakyReLU) of the gate / head MLPs
  * (minkunet.py:165-181,376-380): y = act(x @ W^T + b [+ addend]); W is (n_out, n_in) torch layout.
- * act: 0 none, 1 LeakyReLU(0.1), 2 tanh.  rows read from d_m if non-NULL.
+ * act: 0 none, 1 LeakyReLU(0.1), 2 tanh.  rows read from d_m if non-NULL.  ld_addend >= n_out when addend is given.
  * Optional input transform x' = pre_act(x + prebias[k]) (prebias (n_in) or NULL): evaluates the
  * hoisted gate MLP  latemp(cat(p,t)) = W2 . leaky(Wp.p + (Wt.t + b1)) + b2  (SURVEY.md App. D.1). */
 int lb2_linear(void* h, void* stream, const float* x, int64_t ldx, const float* w, const float* b,
@@ -323,7 +323,8 @@ int lb2_linear(void* h, void* stream, const float* x, int64_t ldx, const float* 
 /* The head of the U-Nets in one pass over the rows — `last` of MinkUNetDiff / MinkUNet (minkunet.py:376-380, :585-588):
  * y = out_act(W1 . LeakyReLU_0.1(W0 . x + b0) + b1), W0 (n_hid, n_in), W1 (n_out, n_hid) in torch layout; out_act as lb2_linear.
  * npass (1 or 2) row blocks x + p * x_pass_stride -> y + p * y_pass_stride (floats) share the weights and the launch.
- * n_in: multiple of 16, <= 128; n_hid <= 64; n_out <= 24; ldx a multiple of 4. */
+ * n_in: multiple of 16, <= 128; n_hid <= 64; n_out <= 24; ldx a multiple of 4; x 16-byte aligned and, with npass 2,
+ * x_pass_stride a multiple of 4 (rows are read with float4 loads). */
 int lb2_head_mlp(void* h, void* stream, const float* x, int64_t ldx, int64_t x_pass_stride, const float* w0, const float* b0,
                  const float* w1, const float* b1, int32_t m_cap, const int32_t* d_m, int32_t n_in, int32_t n_hid,
                  int32_t n_out, int32_t out_act, int32_t npass, float* y, int64_t ldy, int64_t y_pass_stride);

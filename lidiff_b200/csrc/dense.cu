@@ -442,6 +442,7 @@ extern "C" int lb2_linear(void* handle, void* stream, const float* x, int64_t ld
                           const float* prebias, int32_t pre_act) {
     Lb2Handle* h = (Lb2Handle*)handle;
     LB2_REQUIRE(h, h && x && w && y && m_cap > 0 && n_in > 0 && n_out > 0 && ldx >= n_in && ldy >= n_out, "linear");
+    LB2_REQUIRE(h, !addend || ld_addend >= n_out, "linear: ld_addend < n_out");
     dim3 grid(cdiv(m_cap, LIN_BM), cdiv(n_out, LIN_BN));
     k_linear<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, w, b, addend, ld_addend, m_cap, d_m, n_in, n_out, act, y, ldy, prebias, pre_act);
     LB2_POST_LAUNCH(h, "k_linear");
@@ -516,6 +517,8 @@ extern "C" int lb2_head_mlp(void* handle, void* stream, const float* x, int64_t 
     LB2_REQUIRE(h, h && x && w0 && w1 && y && m_cap > 0 && npass >= 1 && npass <= 2, "head_mlp");
     LB2_REQUIRE(h, n_in >= 16 && n_in <= 128 && n_in % 16 == 0 && n_hid >= 1 && n_hid <= 64 && n_out >= 1 && n_out <= 24 && ldx >= n_in &&
                    ldx % 4 == 0 && ldy >= n_out, "head_mlp shape");
+    // every row is read with float4 loads: the base of each pass must be 16-byte aligned
+    LB2_REQUIRE(h, (uintptr_t)x % 16 == 0 && (npass == 1 || x_pass_stride % 4 == 0), "head_mlp: x or x_pass_stride not 16-byte aligned");
     const size_t smem = ((size_t)n_hid * n_in + n_hid + (size_t)n_out * n_hid + n_out) * sizeof(float);
     const dim3 grid((unsigned)std::min<long long>(cdiv(m_cap, 64), (long long)h->num_sms * 8), (unsigned)npass);
     if (n_out <= 4)

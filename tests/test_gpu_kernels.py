@@ -222,43 +222,54 @@ def test_linear_matches_torch(m, n_in, n_out, act):
     assert rel_err(y, ref) < 1e-5
 
 
-@pytest.mark.parametrize("second", [0, 1])
-def test_guidance_dpm_step_bit_exact(second):
-    """given identical eps the fused tail reproduces torch's fp64 evaluation bit for bit (x_next AND coords)"""
+@pytest.mark.parametrize("second,T,i,div_mode,with_eps,batch", [
+    pytest.param(0, 50, 0, 1, True, False, id="0"), pytest.param(1, 50, 7, 1, True, False, id="1"),
+    pytest.param(1, 50, 7, 0, True, False, id="div_mode0"),
+    pytest.param(1, 50, 7, 1, False, True, id="no_eps_out-batch_col"),         # the engine's loop: eps_out None, a batch engine's column
+    pytest.param(1, 50, 49, 1, False, True, id="last_step_T50"),               # second order
+    pytest.param(1, 10, 9, 0, False, False, id="last_step_T10"),               # lower_order_final: first order although x0 is stored
+])
+def test_guidance_dpm_step_bit_exact(second, T, i, div_mode, with_eps, batch):
+    """given identical eps the fused tail reproduces torch's fp64 evaluation bit for bit (x_next AND coords).  `second`: an x0
+    prediction is stored; the update is second order unless it is the last step of fewer than 15 (engine.step's rule)"""
     from lidiff_b200._lib import DpmCoef
     from lidiff_b200.scheduler import DPMSolverMultistepScheduler as S
     n, m = 60_000, 20_000
-    g = torch.Generator().manual_seed(9 + second)
+    g = torch.Generator().manual_seed(9 + second + 100 * (T != 50 or i not in (0, 7)) + 10 * (1 - div_mode) + 20 * batch)
     inv = torch.randint(0, m, (n,), generator=g)
     e_c, e_u = torch.randn(m, 3, generator=g), torch.randn(m, 3, generator=g)
     x_init = torch.randn(1, n, 3, generator=g, dtype=torch.float64) * 20
     x_t = (x_init + torch.randn(1, n, 3, generator=g, dtype=torch.float64)).float()
     noise = torch.randn(1, n, 3, generator=g)
     x0_prev = torch.randn(1, n, 3, generator=g, dtype=torch.float64)
+    bcol = torch.randint(0, 4, (n,), generator=g).float() if batch else None
     o = DPMSolverSDE2M()
-    o.set_timesteps(50)
-    i = 7 if second else 0
+    o.set_timesteps(T)
     if second:
         o.model_outputs = [None, x0_prev.clone()]
         o.lower_order_nums = 1
     eps = (e_u + 6.0 * (e_c - e_u))[inv][None]
     sample = x_t - x_init
     x_next_ref = (x_init + o.step(eps, o.timesteps[i], sample, noise[0][None])).float()
-    coord_ref = ome.quantize(x_next_ref, 0.05, "mul")
+    coord_ref = ome.quantize(x_next_ref, 0.05, "div" if div_mode == 0 else "mul")
     s = S(1000, 3.5e-5, 0.007, "linear", algorithm_type="sde-dpmsolver++", solver_order=2)
-    s.set_timesteps(50)
+    s.set_timesteps(T)
     c = s.coefficients(i)
-    cf = DpmCoef(c["c_sample"], c["c_x0"], c["c_noise"], c["sigma_s"], c["alpha_s"], c.get("inv_r0", 0.0) if second else 0.0,
-                 6.0, 0.05, second, 1, 1)
+    so = int(second and not (i == T - 1 and T < 15))
+    cf = DpmCoef(c["c_sample"], c["c_x0"], c["c_noise"], c["sigma_s"], c["alpha_s"], c.get("inv_r0", 0.0) if so else 0.0,
+                 6.0, 0.05, so, div_mode, 1)
     d = lambda t: t.to(DEV).contiguous()
     x0s = d(x0_prev[0])
     x_next = torch.empty(n, 3, device=DEV)
     coord = torch.empty(n, 4, device=DEV)
-    eps_out = torch.empty(n, 3, device=DEV)
-    H().guidance_dpm_step(d(e_c), d(e_u), d(inv.int()), d(x_t[0]), d(x_init[0]), d(noise[0]), x0s, n, cf, eps_out, x_next, coord)
-    assert torch.equal(eps_out.cpu(), eps[0]), "guidance"
+    eps_out = torch.empty(n, 3, device=DEV) if with_eps else None
+    H().guidance_dpm_step(d(e_c), d(e_u), d(inv.int()), d(x_t[0]), d(x_init[0]), d(noise[0]), x0s, n, cf, eps_out, x_next, coord,
+                          d(bcol) if batch else None)
+    if with_eps:
+        assert torch.equal(eps_out.cpu(), eps[0]), "guidance"
     assert torch.equal(x_next.cpu(), x_next_ref[0]), "x_next"
-    assert torch.equal(coord[:, 1:].cpu(), coord_ref[0]) and (coord[:, 0] == 0).all(), "next coordinates"
+    assert torch.equal(coord[:, 1:].cpu(), coord_ref[0]), "next coordinates"
+    assert torch.equal(coord[:, 0].cpu(), bcol if batch else torch.zeros(n)), "batch column"
     assert torch.equal(x0s.cpu(), o.model_outputs[-1][0]), "multistep state"
 
 
