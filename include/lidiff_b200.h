@@ -380,8 +380,11 @@ int lb2_farthest_point_sample_batched(void* h, void* stream, const double* pts, 
  * metrics.py:70,131-132,153-156).  lb2_pc_tree_build sorts the reference cloud along a Morton curve and builds a box hierarchy
  * over it (`tree`: lb2_pc_tree_bytes(n) bytes, n >= 1); lb2_pc_nn gives, for every query, dist[q] = sqrt(dx^2 + dy^2 + dz^2)
  * (fp64, no FMA contraction) to its nearest reference point and, if idx != NULL, idx[q] = that point's index (lowest index on
- * equal distances).  ~log(n) box tests per query, however far the query is from the cloud.
- * scratch >= lb2_pc_nn_scratch_bytes(nq). */
+ * equal distances).  ~log(n) box tests per query, however far the query is from the cloud.  Only a finite squared distance
+ * counts: a query with a NaN or infinite coordinate does not search, reference points with one are nobody's neighbour, and a query
+ * without a finite squared distance to any point (those, a reference without a finite point, or one whose squared distances all
+ * overflow) gets idx[q] = -1 and dist[q] = +inf.  The results are exact for finite coordinates whose squared distances do not
+ * overflow; non-finite ones never fault.  scratch >= lb2_pc_nn_scratch_bytes(nq). */
 size_t lb2_pc_tree_bytes(int32_t n_cap);
 size_t lb2_pc_nn_scratch_bytes(int32_t nq_cap);
 int lb2_pc_tree_build(void* h, void* stream, const double* pts, int32_t n, void* tree);
@@ -502,7 +505,11 @@ size_t lb2_jsd_scratch_bytes(int64_t n);
 int lb2_jsd(void* h, void* stream, const uint32_t* hist_a, const uint32_t* hist_b, int64_t n, double* out, void* scratch);
 
 /* Per-direction distance statistics (RMSE / Chamfer means, metrics.py:72,134; precision / recall counts, metrics.py:158-165):
- * *sum_out = fp64 sum of the n distances; counts_out[k] = number of distances < thresholds[k] (thresholds ascending, nt <= 4096).
+ * *sum_out = fp64 sum of the n distances; counts_out[k] = number of distances < thresholds[k] (NaN and +inf distances are never
+ * counted).  The thresholds must be ascending and not NaN (each distance is binary-searched among them; other orders give wrong
+ * counts without an error), nt <= 4096.  Summation order, with nblk = max(1, min(ceil(n / 256), 1024)) and every addition one
+ * round-to-nearest fp64 add: thread t of block b sums the elements b 256 + t + k nblk 256 in increasing k from +0; each block
+ * reduces its 256 sums by the tree s[t] += s[t + o], o = 128, 64, ..., 1; the block sums are added from +0 in block order.
  * scratch >= lb2_dist_stats_scratch_bytes(nt). */
 size_t lb2_dist_stats_scratch_bytes(int32_t nt);
 int lb2_dist_stats(void* h, void* stream, const double* dist, int32_t n, const double* thresholds, int32_t nt,

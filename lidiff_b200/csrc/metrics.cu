@@ -171,6 +171,8 @@ __device__ __forceinline__ double pc_box_d2(const float* __restrict__ node, doub
 // one thread per query, queries taken in their Morton order (order[t]) so that a warp searches one neighbourhood.  Depth-first,
 // nearer child first; a subtree is skipped only when its box is strictly farther than the best point so far, so every point at the
 // best distance is seen and the lowest index wins.  Cost ~O(log n) box tests per query however far the query is from the cloud.
+// Only a finite d² is accepted, and a query with a NaN or infinite coordinate does not search (as in k_pc_knn): a query without a
+// finite d² to any point keeps idx -1 and dist +inf.
 __global__ void __launch_bounds__(128) k_pc_query(const double* __restrict__ q, int nq, const int* __restrict__ order,
                                                   const unsigned long long* __restrict__ tree, double* __restrict__ dist,
                                                   int* __restrict__ idx) {
@@ -182,10 +184,10 @@ __global__ void __launch_bounds__(128) k_pc_query(const double* __restrict__ q, 
     const int j = order[t];
     const double qx = __ldg(q + 3 * (size_t)j), qy = __ldg(q + 3 * (size_t)j + 1), qz = __ldg(q + 3 * (size_t)j + 2);
     double best = INFINITY;
-    int best_i = 0x7fffffff;
+    int best_i = -1;
     int st_node[PC_STACK];
     double st_lb[PC_STACK];
-    int sp_n = 1;
+    int sp_n = isfinite(qx) && isfinite(qy) && isfinite(qz) ? 1 : 0;
     st_node[0] = 1; st_lb[0] = pc_box_d2(nodes + 8, qx, qy, qz);
     while (sp_n > 0) {
         --sp_n;
@@ -201,6 +203,7 @@ __global__ void __launch_bounds__(128) k_pc_query(const double* __restrict__ q, 
                 const int pi = (int)pzw.y;
                 if (pi < 0) break;                                   // padding slots are at the end of the last leaves only
                 const double d = pc_d2(__dsub_rn(qx, pxy.x), __dsub_rn(qy, pxy.y), __dsub_rn(qz, pzw.x));
+                // a NaN d fails both tests, and an infinite one too while best = +inf (best_i = -1, so pi < best_i is false)
                 if (d < best || (d == best && pi < best_i)) { best = d; best_i = pi; }
             }
         } else {

@@ -56,7 +56,8 @@ def voxel_edges(voxel_size: float) -> np.ndarray:
 
 def nn_distance(query, ref, return_index: bool = False, device="cuda"):
     """distance of every query point to its nearest point of `ref` (fp64 torch tensor on the device; open3d's
-    compute_point_cloud_distance), and with return_index the index of that point (lowest index on equal distances)"""
+    compute_point_cloud_distance), and with return_index the index of that point (lowest index on equal distances); a query
+    without a finite squared distance to any point of `ref` gets +inf and index -1"""
     h = _lib.get_handle(device)
     q, r = _points(query, h.device), _points(ref, h.device)
     if r.shape[0] == 0:
@@ -114,9 +115,13 @@ def evaluate_scan(gt, pred, thresholds=None, voxel_sizes=VOXEL_SIZES, distances:
             events.setdefault(name, []).append(ev)
 
     dirs = {"both": (("pred_to_gt", p, g), ("gt_to_pred", g, p)), "pred": (("pred_to_gt", p, g),), "none": ()}[distances]
-    thr = torch.as_tensor(thr_np, device=dev)
+    # lb2_dist_stats needs ascending thresholds: count at the sorted non-NaN ones and scatter back, so that any order gives
+    # numpy's (dist < t).sum() per threshold, 0 for a NaN one
+    live = np.argsort(thr_np, kind="stable")
+    live = live[~np.isnan(thr_np[live])]
+    thr = torch.as_tensor(thr_np[live], device=dev)
     sums = torch.zeros(len(dirs), dtype=torch.float64, device=dev)
-    cnts = torch.zeros((len(dirs), thr_np.shape[0]), dtype=torch.int64, device=dev)
+    cnts = torch.zeros((len(dirs), live.shape[0]), dtype=torch.int64, device=dev)
     for k, (_, q, r) in enumerate(dirs):
         mark("nn_build")
         tree = h.pc_tree(r)
@@ -155,7 +160,9 @@ def evaluate_scan(gt, pred, thresholds=None, voxel_sizes=VOXEL_SIZES, distances:
         raise ValueError("evaluate_scan: a cloud has no point inside the [-50, 50] m histogram range")
     for k, (name, _, _) in enumerate(dirs):
         setattr(rec, f"sum_{name}", float(sums[k]))
-        setattr(rec, f"cnt_{name}", cnts[k].astype(np.int64))
+        cnt = np.zeros(thr_np.shape[0], np.int64)
+        cnt[live] = cnts[k]
+        setattr(rec, f"cnt_{name}", cnt)
     rec.conf = conf[: len(voxel_sizes)].astype(np.uint64)
     if hist:
         rec.jsd_3d, rec.jsd_bev = float(jsd[0]), float(jsd[1])
@@ -304,10 +311,12 @@ def record_from_rows(rows: torch.Tensor) -> ScanRecord:
 
 def _nn_sq_dist(q: torch.Tensor, r: torch.Tensor) -> torch.Tensor:
     """((q - r[idx])**2).sum(-1) in q's dtype, idx = the exact (fp64) nearest point of r to every row of q, lowest index on ties.
-    Differentiable in q and r; the gradient of r[idx] is summed per row of r in query order (rowsum.GatherRows), without atomics."""
+    Differentiable in q and r; the gradient of r[idx] is summed per row of r in query order (rowsum.GatherRows), without atomics.
+    A query without a finite squared distance (idx -1: a NaN or infinite query, a reference without a finite point, or an
+    overflowing distance) gathers row 0, whose term is then non-finite too, so the loss is NaN or inf as pytorch3d's would be."""
     with torch.no_grad():
         _, idx = nn_distance(q, r, return_index=True, device=q.device)
-    return ((q - GatherRows.apply(r, idx.long())) ** 2).sum(-1)
+    return ((q - GatherRows.apply(r, idx.long().clamp(min=0))) ** 2).sum(-1)
 
 
 def chamfer_distance(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normals=None, weights=None, batch_reduction="mean",

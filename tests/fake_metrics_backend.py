@@ -5,17 +5,36 @@ import numpy as np
 import torch
 
 import fake_backend
+import metrics_reference
+
+
+class _Tree:
+    """the reference cloud (`data`, every row) and a cKDTree over its finite rows (`kd`, None without any; `live` their indices)"""
+
+    def __init__(self, pts):
+        from scipy.spatial import cKDTree
+        self.data = pts
+        self.live = np.nonzero(np.isfinite(pts).all(1))[0]
+        self.kd = cKDTree(pts[self.live]) if self.live.shape[0] else None
 
 
 class FakeMetricsHandle(fake_backend.FakeHandle):
     def pc_tree(self, pts):
-        from scipy.spatial import cKDTree
         self.launches += 12
-        return cKDTree(pts.numpy())
+        return _Tree(pts.numpy())
 
     def pc_nn(self, q, tree, dist, idx=None):
+        """lb2_pc_nn's contract: a query without a finite squared distance (non-finite, no finite reference point, overflow)
+        gets (+inf, -1)"""
         self.launches += 6
-        d, j = tree.query(q.numpy(), k=1)
+        qn = q.numpy()
+        d, j = np.full(qn.shape[0], np.inf), np.full(qn.shape[0], -1, np.int64)
+        ok = np.isfinite(qn).all(1)
+        if tree.kd is not None and ok.any():
+            kd, kj = tree.kd.query(qn[ok], k=1)
+            found = kd < np.inf                                      # cKDTree: inf and index n for no neighbour
+            d[np.nonzero(ok)[0][found]] = kd[found]
+            j[np.nonzero(ok)[0][found]] = tree.live[kj[found]]
         dist[:] = torch.from_numpy(d)
         if idx is not None:
             idx[:] = torch.from_numpy(j.astype(np.int32))
@@ -63,10 +82,11 @@ class FakeMetricsHandle(fake_backend.FakeHandle):
         out[0] = float(jensenshannon(a / a.sum(), b / b.sum())) if a.sum() and b.sum() else float("nan")
 
     def dist_stats(self, dist, thresholds, sum_out, counts_out):
+        """the kernel's order and its binary search, which counts correctly only for ascending, NaN-free thresholds"""
         self.launches += 2
         d = dist.numpy()
-        sum_out[0] = float(d.sum())
-        counts_out[:] = torch.from_numpy((d[None, :] < thresholds.numpy()[:, None]).sum(1))
+        sum_out[0] = metrics_reference.ordered_sum(d)
+        counts_out[:] = torch.from_numpy(metrics_reference.ds_kernel_counts(d, thresholds.numpy()))
 
 
 def install(monkeypatch):

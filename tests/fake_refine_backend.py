@@ -7,6 +7,7 @@ import numpy as np
 import torch
 
 import fake_backend
+import metrics_reference
 from lidiff_b200 import _lib
 from lidiff_b200.datasets_refine import SEGMENT_DTYPE
 
@@ -97,11 +98,10 @@ class FakeRefineHandle(fake_backend.FakeHandle):
         return pts.numpy().copy()
 
     def pc_nn(self, q, tree, dist, idx=None):
-        """exact nearest neighbour by fp64 brute force, lowest index on ties"""
+        """exact nearest neighbour by fp64 brute force in lb2_pc_nn's order, lowest index on ties, (+inf, -1) without a finite d²"""
         self.launches += 6
-        d2 = ((q.numpy()[:, None, :] - tree[None, :, :]) ** 2).sum(-1)
-        j = d2.argmin(1)
-        dist[:] = torch.from_numpy(np.sqrt(d2[np.arange(len(j)), j]))
+        d, j = metrics_reference.nn(q.numpy(), tree)
+        dist[:] = torch.from_numpy(d)
         if idx is not None:
             idx[:] = torch.from_numpy(j.astype(np.int32))
 
