@@ -625,6 +625,44 @@ size_t lb2_voxel_first_f64_scratch_bytes(int64_t n);
 int lb2_voxel_first_f64(void* h, void* stream, const double* points, int64_t n, double voxel_size, double max_range, double* out,
                         int32_t* d_out, void* scratch);
 
+/* ---- host random streams drawn on the device (rng.cu, lidiff_b200/rng.py) ------------------------------------------------------
+ *
+ * lb2_mt19937_words: the next n tempered MT19937 words of the 624-word state `state` (device uint32[624], updated in place) at
+ * position pos in [0, 624] (numpy's pos; torch's 625 - left; 624 = twist before the next word) -> out (device uint32[n]);
+ * *pos_out (host) = the position afterwards.  One CTA; the twist is the reference MT19937's, word for word.
+ *
+ * lb2_legacy_gauss: numpy's legacy_gauss (the polar method of RandomState.randn) called n_out times over `words` (device, 16-byte
+ * aligned, from lb2_mt19937_words; n_words / 4 attempts) with the incoming cache (has_gauss, gauss) -> out (device fp64[n_out]).
+ * Attempt k reads words 4k .. 4k+3: x = 2 ((w0 >> 5) 2^26 + (w1 >> 6)) 2^-53 - 1 for x1 then x2, r2 = x1 x1 + x2 x2 (no FMA),
+ * rejected when r2 >= 1 or r2 == 0; f = sqrt(-2 log(r2) / r2); outputs f x2, then f x1.  log is glibc's: where the double-double
+ * log of r2 lies more than `band` ulp from a rounding midpoint its leading word is used (glibc's log errs by less than 0.519 ulp,
+ * so it returns the correct rounding there); the other attempts are copied to the host and resolved with libm's log.
+ * band in [0, 0.5] (LB2_GAUSS_BAND by default; 0.5 resolves every attempt on the host).  The call synchronises `stream` (one read
+ * of the attempt and deferred counts, one of the deferred attempts).  *info (host): words_used = the words numpy consumed,
+ * deferred = attempts resolved on the host, (has_gauss, gauss) = numpy's cache afterwards; short_words = 1 when the words held
+ * too few accepted attempts: nothing is valid then, call again with more words of the same stream.
+ * scratch >= lb2_legacy_gauss_scratch_bytes(n_words, n_out).
+ *
+ * lb2_randperm: torch.randperm(n) of the CPU generator: out (device int64[n]) = the identity shuffled by z_i = words[i] % (n - i),
+ * swap(out[i], out[i + z_i]) for i < n - 1 in order (words: device uint32[n - 1] from lb2_mt19937_words), computed in rounds of
+ * deterministic reservations by one cooperative grid.  n < LB2_RANDPERM_MAX_N (torch draws 64-bit words from there: LB2_ERR_ARG).
+ * *d_rounds (device int32, may be NULL) = the reservation rounds.  scratch >= lb2_randperm_scratch_bytes(n). */
+#define LB2_GAUSS_BAND (1.0 / 32.0)
+#define LB2_RANDPERM_MAX_N 214748364LL      /* UINT32_MAX / 20 */
+typedef struct {
+    int64_t words_used;
+    int64_t deferred;
+    int32_t short_words;
+    int32_t has_gauss;
+    double  gauss;
+} Lb2GaussInfo;
+int lb2_mt19937_words(void* h, void* stream, uint32_t* state, int32_t pos, int64_t n, uint32_t* out, int32_t* pos_out);
+size_t lb2_legacy_gauss_scratch_bytes(int64_t n_words, int64_t n_out);
+int lb2_legacy_gauss(void* h, void* stream, const uint32_t* words, int64_t n_words, int64_t n_out, int32_t has_gauss, double gauss,
+                     double band, double* out, Lb2GaussInfo* info, void* scratch);
+size_t lb2_randperm_scratch_bytes(int64_t n);
+int lb2_randperm(void* h, void* stream, const uint32_t* words, int64_t n, int64_t* out, int32_t* d_rounds, void* scratch);
+
 #ifdef __cplusplus
 }
 #endif

@@ -77,6 +77,7 @@ EXPORTS = [
     "lb2_segment_dot_scratch_bytes", "lb2_segment_dot",
     "lb2_sync_bn_max", "lb2_sync_bn_sum", "lb2_sync_bn_sumsq", "lb2_sync_bn_apply",
     "lb2_sync_bn_backward_max", "lb2_sync_bn_backward_sum", "lb2_sync_bn_backward_apply",
+    "lb2_mt19937_words", "lb2_legacy_gauss_scratch_bytes", "lb2_legacy_gauss", "lb2_randperm_scratch_bytes", "lb2_randperm",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -84,6 +85,15 @@ RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
 
 class Pose(C.Structure):
     _fields_ = [("m", C.c_float * 12)]
+
+
+class GaussInfo(C.Structure):
+    _fields_ = [("words_used", C.c_int64), ("deferred", C.c_int64), ("short_words", C.c_int32), ("has_gauss", C.c_int32),
+                ("gauss", C.c_double)]
+
+
+GAUSS_BAND = 1.0 / 32.0             # LB2_GAUSS_BAND: ulp from a rounding midpoint below which log(r2) is taken from the host's libm
+RANDPERM_MAX_N = 214748364          # LB2_RANDPERM_MAX_N = UINT32_MAX // 20
 
 
 class Segment(C.Structure):
@@ -208,6 +218,13 @@ class Lib:
         d.lb2_sync_bn_backward_max.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp]
         d.lb2_sync_bn_backward_sum.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp]
         d.lb2_sync_bn_backward_apply.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, vp]
+        d.lb2_mt19937_words.argtypes = [vp, vp, vp, i32, i64, vp, C.POINTER(i32)]
+        d.lb2_legacy_gauss_scratch_bytes.argtypes = [i64, i64]
+        d.lb2_legacy_gauss_scratch_bytes.restype = C.c_size_t
+        d.lb2_legacy_gauss.argtypes = [vp, vp, vp, i64, i64, i32, f64, f64, vp, C.POINTER(GaussInfo), vp]
+        d.lb2_randperm_scratch_bytes.argtypes = [i64]
+        d.lb2_randperm_scratch_bytes.restype = C.c_size_t
+        d.lb2_randperm.argtypes = [vp, vp, vp, i64, vp, vp, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -588,6 +605,29 @@ class Handle:
         d_out = [rows, status]"""
         self._check(self.dll.lb2_voxel_first_f64(self.hp, self._stream(), _ptr(points), int(points.shape[0]), float(voxel_size),
                                                  float(max_range), _ptr(out), _ptr(d_out), _ptr(scratch)), "lb2_voxel_first_f64")
+
+    # -- host random streams on the device (lidiff_b200.rng) ----------------------------------------------------------------------
+    def mt19937_words(self, state, pos, n, out) -> int:
+        """out[:n] = the next n tempered MT19937 words of `state` (device int32 (624,), updated in place) at numpy position `pos`;
+        returns the position afterwards"""
+        pos_out = C.c_int32()
+        self._check(self.dll.lb2_mt19937_words(self.hp, self._stream(), _ptr(state), int(pos), int(n), _ptr(out), C.byref(pos_out)),
+                    "lb2_mt19937_words")
+        return int(pos_out.value)
+
+    def legacy_gauss(self, words, n_words, n_out, has_gauss, gauss, band, out) -> GaussInfo:
+        """numpy's legacy_gauss n_out times over the first n_words of `words` -> out (fp64); synchronises the stream"""
+        info = GaussInfo()
+        scratch = self._bytes(self.dll.lb2_legacy_gauss_scratch_bytes(int(n_words), int(n_out)))
+        self._check(self.dll.lb2_legacy_gauss(self.hp, self._stream(), _ptr(words), int(n_words), int(n_out), int(has_gauss), float(gauss),
+                                              float(band), _ptr(out), C.byref(info), _ptr(scratch)), "lb2_legacy_gauss")
+        return info
+
+    def randperm(self, words, n, out, d_rounds=None):
+        """out (int64 (n,)) = torch's CPU randperm(n) shuffle driven by the n - 1 words `words`"""
+        scratch = self._bytes(self.dll.lb2_randperm_scratch_bytes(int(n)))
+        self._check(self.dll.lb2_randperm(self.hp, self._stream(), _ptr(words), int(n), _ptr(out), _ptr(d_rounds), _ptr(scratch)),
+                    "lb2_randperm")
 
 
 _LIB = None

@@ -27,7 +27,7 @@ import numpy as np
 import torch
 from torch.utils.data import DataLoader, Dataset
 
-from . import _lib
+from . import _lib, rng
 from .kitti import label_path, load_poses, natural_sorted, read_labels, read_scan
 from .pipeline import FPS_CLUSTER_MIN_SCANS
 from .preprocess import farthest_point_sample, farthest_point_sample_batched
@@ -81,7 +81,7 @@ def repeat_rows(p: torch.Tensor, times: int) -> torch.Tensor:
 
 class TemporalKITTISet(Dataset):
     def __init__(self, data_dir, seqs, split, resolution, num_points, max_range, dataset_norm=False, std_axis_norm=False,
-                 device="cuda"):
+                 device="cuda", device_rng=False):
         super().__init__()
         self.data_dir = data_dir
         self.n_clusters = 50
@@ -90,6 +90,7 @@ class TemporalKITTISet(Dataset):
         self.max_range = max_range
         self.split = split
         self.seqs = seqs
+        self.device_rng = device_rng          # the map crop's torch randperm drawn on the GPU (lidiff_b200.rng), the same values
         self.h = _lib.get_handle(device)
         self.device = self.h.device
         self.cache_maps = {}
@@ -182,7 +183,8 @@ class TemporalKITTISet(Dataset):
             raise ValueError(f"{path}: the partial scan spans more than 2^21 viewpoint cells along an axis")
         if n_in == 0:
             raise ValueError(f"{path}: no point of the ground-truth map lies in the partial scan's {VIEWPOINT_VOXEL:g} m viewpoint grid")
-        perm = torch.randperm(n_in)                               # torch's global CPU generator, as collations.py:54
+        # torch's global CPU generator, as collations.py:54
+        perm = rng.torch_randperm(n_in, device=self.device) if self.device_rng else torch.randperm(n_in)
         times = int(np.ceil(self.num_points / n_in))
         rows = perm.to(self.device)[torch.arange(self.num_points, device=self.device) // times]
         p_full = inc[:n_in][rows]
@@ -232,9 +234,11 @@ class TemporalKittiDataModule:
     """The reference's data module: its splits, batch sizes and shuffle flags.  The loaders yield batches in the main process
     (the samples are built on the GPU, which worker processes cannot share), so the configured num_workers is not used."""
 
-    def __init__(self, cfg, device="cuda"):
+    def __init__(self, cfg, device="cuda", device_rng=None):
         self.cfg = cfg
         self.device = device
+        # the map crop's torch randperm drawn on the GPU (lidiff_b200.rng), the same values; None: the config's data.device_rng (default off)
+        self.device_rng = bool(cfg["data"].get("device_rng", False)) if device_rng is None else bool(device_rng)
 
     def prepare_data(self):
         pass
@@ -246,7 +250,7 @@ class TemporalKittiDataModule:
         d = self.cfg["data"]
         return TemporalKITTISet(data_dir=d["data_dir"], seqs=seqs, split=split, resolution=d["resolution"], num_points=d["num_points"],
                                 max_range=d["max_range"], dataset_norm=d["dataset_norm"], std_axis_norm=d["std_axis_norm"],
-                                device=self.device)
+                                device=self.device, device_rng=self.device_rng)
 
     def train_dataloader(self):
         return DataLoader(self._set(self.cfg["data"]["train"], self.cfg["data"]["split"]), batch_size=self.cfg["train"]["batch_size"],

@@ -27,7 +27,7 @@ import numpy as np
 import torch
 from torch.utils.data import DataLoader, Dataset
 
-from . import _lib
+from . import _lib, rng
 from .datasets import SparseSegmentCollation, augment, repeat_rows
 from .kitti import label_path, load_poses, read_labels, read_scan
 
@@ -57,7 +57,7 @@ def repeat_to(rows: torch.Tensor, perm: torch.Tensor, n: int) -> torch.Tensor:
 
 
 class TemporalKITTISet(Dataset):
-    def __init__(self, data_dir, scan_window, seqs, split, resolution, num_points, mode, device="cuda"):
+    def __init__(self, data_dir, scan_window, seqs, split, resolution, num_points, mode, device="cuda", device_rng=False):
         super().__init__()
         self.data_dir = data_dir
         self.n_clusters = 50
@@ -67,6 +67,7 @@ class TemporalKITTISet(Dataset):
         self.split = split
         self.seqs = seqs
         self.mode = mode
+        self.device_rng = device_rng          # numpy's randn and torch's randperms drawn on the GPU (lidiff_b200.rng), the same values
         self.h = _lib.get_handle(device)
         self.device = self.h.device
         self.datapath_list()
@@ -140,7 +141,10 @@ class TemporalKITTISet(Dataset):
         if self.split == "train":
             p_concat = augment(p_concat)
         n = p_concat.shape[0]
-        r = torch.from_numpy(np.random.randn(1, n, 3)[0]).to(self.device)      # numpy's global generator, every row
+        if self.device_rng:                                                     # numpy's global generator, every row
+            r = rng.numpy_randn(1, n, 3, device=self.device)[0]
+        else:
+            r = torch.from_numpy(np.random.randn(1, n, 3)[0]).to(self.device)
         noise = torch.empty((n, 3), dtype=torch.float64, device=self.device)
         full = torch.empty((n, 3), dtype=torch.float64, device=self.device)
         counts = torch.zeros(3, dtype=torch.int32, device=self.device)
@@ -152,8 +156,9 @@ class TemporalKITTISet(Dataset):
             raise ValueError(f"{where}: a point's {DEDUP_VOXEL:g} m voxel index is outside +-2^20")
         if n_full == 0 or n_noise == 0:
             raise ValueError(f"{where}: no {'ground-truth' if n_full == 0 else 'noisy'} point lies within {MAX_RANGE:g} m")
-        perm_full = torch.randperm(n_full)                       # torch's global CPU generator, collations.py:31, :34
-        perm_noise = torch.randperm(n_noise)
+        randperm = (lambda k: rng.torch_randperm(k, device=self.device)) if self.device_rng else torch.randperm
+        perm_full = randperm(n_full)                             # torch's global CPU generator, collations.py:31, :34
+        perm_noise = randperm(n_noise)
         p_full = repeat_to(full[:n_full], perm_full, 2 * self.num_points)
         p_noise = repeat_to(noise[:n_noise], perm_noise, self.num_points)
         return [p_full, p_full.mean(0), p_full.std(0), p_noise, window]
@@ -168,9 +173,11 @@ class TemporalKittiDataModule:
     (datasets_refine.py:58-71).  The loaders yield batches in the main process (the samples are built on the GPU, which worker
     processes cannot share), so the configured num_workers is not used."""
 
-    def __init__(self, cfg, device="cuda"):
+    def __init__(self, cfg, device="cuda", device_rng=None):
         self.cfg = cfg
         self.device = device
+        # numpy's randn and torch's randperms drawn on the GPU (lidiff_b200.rng), the same values; None: the config's data.device_rng (default off)
+        self.device_rng = bool(cfg["data"].get("device_rng", False)) if device_rng is None else bool(device_rng)
 
     def prepare_data(self):
         pass
@@ -181,7 +188,8 @@ class TemporalKittiDataModule:
     def _loader(self, seqs, split, mode, batch_size, shuffle=False):
         d = self.cfg["data"]
         ds = TemporalKITTISet(data_dir=d["data_dir"], scan_window=d["scan_window"], seqs=seqs, split=split, resolution=d["resolution"],
-                              num_points=d["num_points"], mode=mode, device=self.device)
+                              num_points=d["num_points"], mode=mode, device=self.device,
+                              device_rng=self.device_rng)
         return DataLoader(ds, batch_size=batch_size, shuffle=shuffle, num_workers=0, collate_fn=SparseSegmentCollation("refine"))
 
     def train_dataloader(self):

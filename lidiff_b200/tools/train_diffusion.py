@@ -166,7 +166,8 @@ def load_checkpoint(path, nets, opt=None, sched=None):
 @click.option("--checkpoint", "-ckpt", type=str, default=None, help="resume training from this checkpoint (.ckpt)")
 @click.option("--out", type=str, default=None, help="checkpoint directory (default experiments/<experiment.id>/checkpoints)")
 @click.option("--max-steps", type=int, default=None, help="stop this run after this many optimiser steps")
-def main(config, weights, checkpoint, out, max_steps):
+@click.option("--device-rng", is_flag=True, help="draw the samples' numpy randn / torch randperm on the GPU, bit for bit (lidiff_b200.rng; also data.device_rng: true in the config)")
+def main(config, weights, checkpoint, out, max_steps, device_rng):
     set_deterministic()
     run = ddp.start()
     with open(config) as f:
@@ -193,7 +194,7 @@ def main(config, weights, checkpoint, out, max_steps):
     model.train()
     if run.main:
         print("TRAINING MODE")
-    dm = TemporalKittiDataModule(cfg, device=device)
+    dm = TemporalKittiDataModule(cfg, device=device, device_rng=True if device_rng else None)
     train_loader = ddp.sharded(dm.train_dataloader(), run, shuffle=True)
     val_loader = ddp.sharded(dm.val_dataloader(), run, shuffle=False)
     last_step = None if max_steps is None else step + max_steps
