@@ -663,6 +663,45 @@ int lb2_legacy_gauss(void* h, void* stream, const uint32_t* words, int64_t n_wor
 size_t lb2_randperm_scratch_bytes(int64_t n);
 int lb2_randperm(void* h, void* stream, const uint32_t* words, int64_t n, int64_t* out, int32_t* d_rounds, void* scratch);
 
+/* ---- point-cloud images without a display (render.cu, lidiff_b200/render.py) — the view of lidiff/vis_pcd.py's
+ * o3d.visualization.draw_geometries as an 8-bit RGB image.  Every fp64 operation below is rounded on its own (no FMA contraction)
+ * and dot products are summed left to right, a.b = (a.x b.x + a.y b.y) + a.z b.z, so a sequential host evaluation gives the same keys
+ * and colours bit for bit.  Both calls are deterministic and use no float atomics.
+ *
+ * Camera (lb2_render_camera; the caller computes every transcendental): F = normalize(front), right = normalize(up x F),
+ * up' = normalize(F x right), eye = lookat + F distance, with normalize(a) = a / sqrt(a.a) per component and
+ * a x b = (a.y b.z - a.z b.y, a.z b.x - a.x b.z, a.x b.y - a.y b.x).  focal = (height / 2) / tan(fov / 2) in pixels.
+ *
+ * lb2_render_splat: for point p (fp64 (n, 3), n < 2^32 - 1) with d = p - eye:
+ *   depth = -(d.F),  u = width / 2 + (focal (d.right)) / depth,  v = height / 2 - (focal (d.up')) / depth.
+ * Skipped: a NaN / inf coordinate, depth <= 1e-3 distance (no far plane), a NaN u or v.  With a = u - s/2, b = u + s/2 (s = point_size,
+ * each rounded), each clamped to [-1, width + 1], the point covers the columns c in [0, width) with a <= c + 0.5 < b, i.e.
+ * ceil(a - 0.5) <= c < ceil(b - 0.5); rows likewise from v and height.  An integer s therefore covers s x s pixels, as an OpenGL square
+ * point of that size does.  Each covered pixel takes atomicMin(keys[row width + col], (float_bits(float(depth)) << 32) | index): the
+ * nearest point wins and ties go to the lower index, whatever the launch order.  keys (device uint64[height width]) must be filled
+ * with LB2_KEY_EMPTY (background) by the caller; several splats may accumulate into one buffer.  0 < point_size <= 4096.
+ *
+ * lb2_render_shade: rgb (device uint8[height][width][3]) from the keys.  Background: (255, 255, 255).  Otherwise, with i = the key's
+ * index: the base colour c is float(colors[i]) (colors fp64 (n, 3), NULL: none) or open3d's ColorMapJet of
+ * t = (z_i - z_lo) / (z_hi - z_lo) clamped to [0, 1] (t = 0 when z_hi == z_lo): c = (jet(2t - 1.5), jet(2t - 1.0), jet(2t - 0.5)) in fp64 with
+ *   jet(x) = 0 (x <= -0.75), ((x + 0.75) / 0.5) 1 + 0 (x <= -0.25), 1 (x <= 0.25), ((x - 0.25) / 0.5) (-1) + 1 (x <= 0.75), else 0,
+ * each channel rounded to fp32.  With normals (fp64 (n, 3), NULL: none) the two-sided headlight factor
+ * k = 0.25f + 0.75f |float(n_i.F)| in fp32 (k = 1 when float(n_i.F) is not finite), else k = 1.  Each channel:
+ * rint(255f clamp(c k, 0, 1)) in fp32, round half to even, where clamp maps NaN to 0.  A point whose pixels are all covered by
+ * nearer points is never read. */
+typedef struct {
+    double  lookat[3];
+    double  front[3];       /* from the look-at point towards the eye; need not be unit length, must not be zero */
+    double  up[3];
+    double  distance;       /* > 0 */
+    double  focal;          /* > 0, pixels */
+    int32_t width, height;  /* > 0 */
+} lb2_render_camera;
+int lb2_render_splat(void* h, void* stream, const double* pts, int64_t n, const lb2_render_camera* cam, double point_size,
+                     uint64_t* keys);
+int lb2_render_shade(void* h, void* stream, const uint64_t* keys, const double* pts, const double* normals, const double* colors,
+                     double z_lo, double z_hi, const lb2_render_camera* cam, uint8_t* rgb);
+
 #ifdef __cplusplus
 }
 #endif

@@ -78,6 +78,7 @@ EXPORTS = [
     "lb2_sync_bn_max", "lb2_sync_bn_sum", "lb2_sync_bn_sumsq", "lb2_sync_bn_apply",
     "lb2_sync_bn_backward_max", "lb2_sync_bn_backward_sum", "lb2_sync_bn_backward_apply",
     "lb2_mt19937_words", "lb2_legacy_gauss_scratch_bytes", "lb2_legacy_gauss", "lb2_randperm_scratch_bytes", "lb2_randperm",
+    "lb2_render_splat", "lb2_render_shade",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -94,6 +95,11 @@ class GaussInfo(C.Structure):
 
 GAUSS_BAND = 1.0 / 32.0             # LB2_GAUSS_BAND: ulp from a rounding midpoint below which log(r2) is taken from the host's libm
 RANDPERM_MAX_N = 214748364          # LB2_RANDPERM_MAX_N = UINT32_MAX // 20
+
+
+class RenderCamera(C.Structure):
+    _fields_ = [("lookat", C.c_double * 3), ("front", C.c_double * 3), ("up", C.c_double * 3), ("distance", C.c_double),
+                ("focal", C.c_double), ("width", C.c_int32), ("height", C.c_int32)]
 
 
 class Segment(C.Structure):
@@ -225,6 +231,8 @@ class Lib:
         d.lb2_randperm_scratch_bytes.argtypes = [i64]
         d.lb2_randperm_scratch_bytes.restype = C.c_size_t
         d.lb2_randperm.argtypes = [vp, vp, vp, i64, vp, vp, vp]
+        d.lb2_render_splat.argtypes = [vp, vp, vp, i64, C.POINTER(RenderCamera), f64, vp]
+        d.lb2_render_shade.argtypes = [vp, vp, vp, vp, vp, vp, f64, f64, C.POINTER(RenderCamera), vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -628,6 +636,18 @@ class Handle:
         scratch = self._bytes(self.dll.lb2_randperm_scratch_bytes(int(n)))
         self._check(self.dll.lb2_randperm(self.hp, self._stream(), _ptr(words), int(n), _ptr(out), _ptr(d_rounds), _ptr(scratch)),
                     "lb2_randperm")
+
+    # -- point-cloud images (lidiff_b200.render) ----------------------------------------------------------------------------------
+    def render_splat(self, pts, cam: RenderCamera, point_size, keys):
+        """keys (uint64 as int64 (height width,), filled with -1 first) <- atomicMin of (float depth bits << 32 | index) over the
+        pixels each point of the fp64 (n, 3) `pts` covers"""
+        self._check(self.dll.lb2_render_splat(self.hp, self._stream(), _ptr(pts), int(pts.shape[0]), C.byref(cam), float(point_size),
+                                              _ptr(keys)), "lb2_render_splat")
+
+    def render_shade(self, keys, pts, normals, colors, z_lo, z_hi, cam: RenderCamera, rgb):
+        """rgb (uint8 (height, width, 3)) from the keys: white background, colours or jet of z, the headlight of the normals"""
+        self._check(self.dll.lb2_render_shade(self.hp, self._stream(), _ptr(keys), _ptr(pts), _ptr(normals), _ptr(colors), float(z_lo),
+                                              float(z_hi), C.byref(cam), _ptr(rgb)), "lb2_render_shade")
 
 
 _LIB = None

@@ -839,12 +839,21 @@ class DenoiseEngine:
         """kernels launched on behalf of this engine's handle: eager launches counted by the library + graph-replayed ones"""
         return self.h.launch_count() - self._captured_launches + self.replayed_launches
 
-    def run(self, x_init: torch.Tensor, x_feats: torch.Tensor, step_noise=None, n_steps=None, return_device=False, fresh=True):
+    def run(self, x_init: torch.Tensor, x_feats: torch.Tensor, step_noise=None, n_steps=None, return_device=False, fresh=True,
+            snapshot_steps=None):
         """x_init (1,N,3) fp64 conditioning scan, x_feats (1,N,3) noisy start ((B,N,3) each for a batch engine, step_noise
-        (T,B,N,3)).  Returns final x_t.F (N,3) ((B*N,3), scan b in rows b*N..)."""
+        (T,B,N,3)).  Returns final x_t.F (N,3) ((B*N,3), scan b in rows b*N..).  snapshot_steps (step counts k in [0, T]): also
+        return {k: a device copy of x_t after k steps} (k = 0: the noisy start), taken on the stream between steps, so no step
+        graph or launch changes; the result is then (x_t, snapshots)."""
         dev, N = self.device, self.N
-        st = self.start(x_init, x_feats, fresh=fresh)
         T = self.T if n_steps is None else n_steps
+        keep = None if snapshot_steps is None else {int(k) for k in snapshot_steps}
+        if keep is not None and not all(0 <= k <= T for k in keep):
+            raise ValueError(f"snapshot_steps must lie in [0, {T}], got {sorted(keep)}")
+        st = self.start(x_init, x_feats, fresh=fresh)
+        snaps = None if keep is None else {}
+        if keep is not None and 0 in keep:
+            snaps[0] = st["xa"].clone()
         if step_noise is not None:
             step_noise = step_noise.reshape(-1, self.cap, 3).to(device=dev, dtype=torch.float32).contiguous()
         for i in range(T):
@@ -853,12 +862,14 @@ class DenoiseEngine:
             # a batch draws (B, N, 3) once per step, as diffusers' step() does inside the reference's batched p_sample_loop
             nz = step_noise[i] if step_noise is not None else torch.randn((self.B, N, 3), device=dev, dtype=torch.float32).reshape(-1, 3)
             self.advance(st, nz)
+            if keep is not None and i + 1 in keep:
+                snaps[i + 1] = st["xa"].clone()
         if return_device:
-            return st["xa"]
+            return st["xa"] if snaps is None else (st["xa"], snaps)
         out = st["xa"].cpu().numpy()
         if self.h.read_status() & 1:
             raise RuntimeError("lidiff_b200: a coordinate left the supported key range during sampling")
-        return out
+        return out if snaps is None else (out, snaps)
 
     # ---- after the loop: postprocess_scan + refinement forward + 6x offsets (pipeline:107-138) ------------------------------
     def postprocess(self, completed: torch.Tensor, x_init: torch.Tensor) -> torch.Tensor:
@@ -903,16 +914,20 @@ class DenoiseEngine:
         h.gather_rows(off_v, g.inv[0], n, 18, out)
         return out
 
-    def complete(self, x_init: torch.Tensor, x_feats: torch.Tensor, step_noise=None, fresh=True):
+    def complete(self, x_init: torch.Tensor, x_feats: torch.Tensor, step_noise=None, fresh=True, snapshot_steps=None):
         """complete_scan after preprocessing (pipeline:117-132), all on the device: T denoising steps, postprocess, refinement
-        forward, 6 offsets per point.  Returns (refined (6n,3), post (n,3)) device tensors."""
-        x_t = self.run(x_init, x_feats, step_noise, return_device=True, fresh=fresh)
+        forward, 6 offsets per point.  Returns (refined (6n,3), post (n,3)) device tensors; with snapshot_steps (see run) also the
+        snapshots: (refined, post, {k: x_t after k steps})."""
+        x_t = self.run(x_init, x_feats, step_noise, return_device=True, fresh=fresh, snapshot_steps=snapshot_steps)
+        snaps = None
+        if snapshot_steps is not None:
+            x_t, snaps = x_t
         post = self.postprocess(x_t, x_init.reshape(-1, 3).to(self.device))
         off = self.refine_offsets(post).reshape(-1, 6, 3)
         refined = (post[:, None, :] + off).reshape(-1, 3)
         if self.h.read_status() & 1:
             raise RuntimeError("lidiff_b200: a coordinate left the supported key range during sampling")
-        return refined, post
+        return (refined, post) if snaps is None else (refined, post, snaps)
 
     def postprocess_batch(self, completed: torch.Tensor, x_init: torch.Tensor):
         """postprocess() of every scan of a batch without a host synchronisation: completed (B*N,3) fp32, x_init (B,N,3) fp64 ->

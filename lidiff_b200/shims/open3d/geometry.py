@@ -110,6 +110,17 @@ class PointCloud(Geometry):
     def has_normals(self):
         return len(self._normals) == len(self._points) > 0
 
+    def has_colors(self):
+        return len(self._colors) == len(self._points) > 0
+
+    def paint_uniform_color(self, color):
+        """every point gets the RGB `color` (3 values in [0, 1])"""
+        c = np.asarray(color, dtype=np.float64).reshape(-1)
+        if c.shape != (3,):
+            raise ValueError(f"paint_uniform_color: expected 3 values, got {color!r}")
+        self._colors = Vector3dVector(np.broadcast_to(c, (len(self._points), 3)).copy())
+        return self
+
     def __repr__(self):
         return f"PointCloud with {len(self._points)} points."
 
