@@ -380,7 +380,9 @@ int lb2_farthest_point_sample_batched(void* h, void* stream, const double* pts, 
  * metrics.py:70,131-132,153-156).  lb2_pc_tree_build sorts the reference cloud along a Morton curve and builds a box hierarchy
  * over it (`tree`: lb2_pc_tree_bytes(n) bytes, n >= 1); lb2_pc_nn gives, for every query, dist[q] = sqrt(dx^2 + dy^2 + dz^2)
  * (fp64, no FMA contraction) to its nearest reference point and, if idx != NULL, idx[q] = that point's index (lowest index on
- * equal distances).  ~log(n) box tests per query, however far the query is from the cloud.  Only a finite squared distance
+ * equal distances).  ~log(n) box tests per query, however far the query is from the cloud.  Rows with a NaN or infinite
+ * coordinate do not affect the tree's shape or the search cost: they are left out of its bounding box and node boxes and sorted
+ * after every finite row (a finite outlier still coarsens the Morton grid; the results stay exact).  Only a finite squared distance
  * counts: a query with a NaN or infinite coordinate does not search, reference points with one are nobody's neighbour, and a query
  * without a finite squared distance to any point (those, a reference without a finite point, or one whose squared distances all
  * overflow) gets idx[q] = -1 and dist[q] = +inf.  The results are exact for finite coordinates whose squared distances do not
@@ -476,7 +478,8 @@ int lb2_sync_bn_backward_apply(void* h, void* stream, const float* dy, const flo
  *   lb2_pc_normals  normals[i] (double[n][3]) = FastEigen3x3 of the one-pass cumulant covariance of the k neighbours idx[i][0..k)
  *                   (idx: int32[n][k], k = the k_eff of lb2_pc_knn): sums of x, y, z, xx, xy, xz, yy, yz, zz in neighbour order,
  *                   divided by k, C = E[pp^T] - E[p]E[p]^T (the identity when k < 3); the eigenvector of the smallest eigenvalue,
- *                   unoriented, (0, 0, 1) where the solver gives the zero vector, NaN where the row holds an index outside
+ *                   unoriented, (0, 0, 1) where the solver gives the zero vector or C has a NaN or infinite entry (the
+ *                   cumulants overflow once a neighbourhood's coordinates pass ~1e154), NaN where the row holds an index outside
  *                   [0, n) (an empty lb2_pc_knn slot; nothing is read for it).  Every operation is rounded on its own, so C is
  *                   bit-exact against a sequential host evaluation and the normal differs from one only through acos / cos. */
 int lb2_pc_knn(void* h, void* stream, const void* tree, int32_t n, int32_t k, int32_t* idx, double* d2);

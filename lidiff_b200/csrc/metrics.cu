@@ -8,18 +8,22 @@
 // point-cloud tree: the reference cloud sorted along a Morton curve (10 bits per axis of the cubic cell grid spanning its bounding
 // box), leaves of PC_LEAF consecutive sorted points, a complete binary tree in heap order whose node boxes are fp32, rounded outward
 // from the fp64 bounds of their points.  The quantisation only orders the points; the search is exact in fp64 (k_pc_query).
+// A row with a NaN or infinite coordinate is nobody's neighbour and does not shape the tree: it is left out of the bounding box and
+// the leaf boxes, and its Morton code (bit 30) sorts it after every finite row, so the grid and the boxes are those of the finite
+// rows alone and a leaf of such rows is an empty box that no search visits.
 // Buffer layout: header (bounding box as order-preserving uint64 keys [6], nleaf, n) | nodes float[2*nleaf][8] {lo xyz, 0, hi xyz, 0}
 //                | sorted points double4[nleaf*PC_LEAF] (x, y, z, original index; index -1 past the last point) | build scratch.
 // ---------------------------------------------------------------------------------------------------
 #define PC_LEAF 8
 #define PC_HDR 64                                   // bytes
 #define PC_STACK 64
-#define PC_BITS 10                                  // Morton bits per axis: 30-bit codes, 4 radix passes
+#define PC_BITS 10                                  // Morton bits per axis: 30-bit codes
+#define PC_SORT_BITS (3 * PC_BITS + 1)              // + bit 30 for rows with a non-finite coordinate: still 4 radix passes of 9 bits
 
 static int pc_nleaf(int n_cap) { int n = 1; while ((long long)n * PC_LEAF < n_cap) n <<= 1; return n; }
 static size_t pc_nodes_bytes(int nleaf) { return (size_t)2 * nleaf * 8 * sizeof(float); }
 static size_t pc_points_bytes(int nleaf) { return (size_t)nleaf * PC_LEAF * sizeof(double4); }
-static size_t pc_sort_bytes(int n_cap) { return 2 * (size_t)n_cap * sizeof(int) + rs_sort_scratch_bytes(n_cap, 3 * PC_BITS); }
+static size_t pc_sort_bytes(int n_cap) { return 2 * (size_t)n_cap * sizeof(int) + rs_sort_scratch_bytes(n_cap, PC_SORT_BITS); }
 
 extern "C" size_t lb2_pc_tree_bytes(int32_t n_cap) {
     if (n_cap <= 0) return 0;
@@ -42,12 +46,17 @@ __global__ void k_pc_init(unsigned long long* __restrict__ hdr, int nleaf, int n
     if (threadIdx.x == 0) { int* hi = (int*)(hdr + 6); hi[0] = nleaf; hi[1] = n; }
 }
 
+__device__ __forceinline__ bool pc_finite(double x, double y, double z) { return isfinite(x) && isfinite(y) && isfinite(z); }
+
+// bounding box of the rows whose three coordinates are finite (none: lo and hi keep their initial keys, which unkey to NaN)
 __global__ void k_pc_bbox(const double* __restrict__ p, int n, unsigned long long* __restrict__ hdr) {
     unsigned long long lo[3] = {~0ull, ~0ull, ~0ull}, hi[3] = {0ull, 0ull, 0ull};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const double v[3] = {__ldg(p + 3 * (size_t)i), __ldg(p + 3 * (size_t)i + 1), __ldg(p + 3 * (size_t)i + 2)};
+        if (!pc_finite(v[0], v[1], v[2])) continue;
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
-            const unsigned long long k = pc_okey(__ldg(p + 3 * (size_t)i + a));
+            const unsigned long long k = pc_okey(v[a]);
             lo[a] = min(lo[a], k); hi[a] = max(hi[a], k);
         }
     }
@@ -71,20 +80,20 @@ __device__ __forceinline__ unsigned pc_spread10(unsigned v) {      // 10 bits ->
     return v;
 }
 
-// Morton code of each point in the cubic grid over the tree's bounding box (points outside it, i.e. queries, are clamped to its faces)
+// Morton code of each point in the cubic grid over the tree's bounding box (points outside it, i.e. queries, are clamped to its faces);
+// a point with a NaN or infinite coordinate gets 1 << 30, above every finite point's code
 __global__ void k_pc_morton(const double* __restrict__ p, int n, const unsigned long long* __restrict__ hdr, unsigned* __restrict__ codes) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const double v[3] = {__ldg(p + 3 * (size_t)i), __ldg(p + 3 * (size_t)i + 1), __ldg(p + 3 * (size_t)i + 2)};
+    if (!pc_finite(v[0], v[1], v[2])) { codes[i] = 1u << (3 * PC_BITS); return; }
     double lo[3], ext = 0.0;
 #pragma unroll
     for (int a = 0; a < 3; ++a) { lo[a] = pc_unkey(hdr[a]); ext = fmax(ext, pc_unkey(hdr[3 + a]) - lo[a]); }
     const double scale = ext > 0.0 ? (double)((1 << PC_BITS) - 1) / ext : 0.0;
     unsigned c[3];
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        const double v = (__ldg(p + 3 * (size_t)i + a) - lo[a]) * scale;
-        c[a] = (unsigned)fmin(fmax(v, 0.0), (double)((1 << PC_BITS) - 1));          // NaN -> 0
-    }
+    for (int a = 0; a < 3; ++a) c[a] = (unsigned)fmin(fmax((v[a] - lo[a]) * scale, 0.0), (double)((1 << PC_BITS) - 1));  // NaN -> 0
     codes[i] = pc_spread10(c[0]) | (pc_spread10(c[1]) << 1) | (pc_spread10(c[2]) << 2);
 }
 
@@ -96,7 +105,8 @@ __global__ void k_pc_gather(const double* __restrict__ p, int n, const int* __re
     sp[i] = make_double4(__ldg(p + 3 * (size_t)j), __ldg(p + 3 * (size_t)j + 1), __ldg(p + 3 * (size_t)j + 2), (double)j);
 }
 
-// leaf boxes: fp32 bounds rounded outward from the fp64 extremes, so every point lies inside its leaf's box; an empty leaf has lo > hi
+// leaf boxes: fp32 bounds rounded outward from the fp64 extremes, so every finite point lies inside its leaf's box; points with a
+// non-finite coordinate are left out, and a leaf without a finite point has lo > hi (an empty box)
 __global__ void k_pc_leaves(const double4* __restrict__ sp, int n, int nleaf, float* __restrict__ nodes) {
     const int l = blockIdx.x * blockDim.x + threadIdx.x;
     if (l >= nleaf) return;
@@ -105,6 +115,7 @@ __global__ void k_pc_leaves(const double4* __restrict__ sp, int n, int nleaf, fl
         const int i = l * PC_LEAF + t;
         if (i >= n) break;
         const double4 q = sp[i];
+        if (!pc_finite(q.x, q.y, q.z)) continue;
         lo[0] = fmin(lo[0], q.x); lo[1] = fmin(lo[1], q.y); lo[2] = fmin(lo[2], q.z);
         hi[0] = fmax(hi[0], q.x); hi[1] = fmax(hi[1], q.y); hi[2] = fmax(hi[2], q.z);
     }
@@ -142,7 +153,7 @@ extern "C" int lb2_pc_tree_build(void* handle, void* stream, const double* pts, 
     LB2_POST_LAUNCH(h, "k_pc_bbox");
     k_pc_morton<<<cdiv(n, 256), 256, 0, s>>>(pts, n, hdr, codes);
     LB2_POST_LAUNCH(h, "k_pc_morton");
-    const int rc = rs_sort_keys(h, s, codes, nullptr, n, 3 * PC_BITS, order, order + n);
+    const int rc = rs_sort_keys(h, s, codes, nullptr, n, PC_SORT_BITS, order, order + n);
     if (rc != LB2_OK) return rc;
     k_pc_gather<<<cdiv(slots, 256), 256, 0, s>>>(pts, n, order, slots, sp);
     LB2_POST_LAUNCH(h, "k_pc_gather");
@@ -229,7 +240,7 @@ extern "C" int lb2_pc_nn(void* handle, void* stream, const double* q, int32_t nq
     int* order = (int*)(codes + nq);
     k_pc_morton<<<cdiv(nq, 256), 256, 0, s>>>(q, nq, hdr, codes);
     LB2_POST_LAUNCH(h, "k_pc_morton");
-    const int rc = rs_sort_keys(h, s, codes, nullptr, nq, 3 * PC_BITS, order, order + nq);
+    const int rc = rs_sort_keys(h, s, codes, nullptr, nq, PC_SORT_BITS, order, order + nq);
     if (rc != LB2_OK) return rc;
     k_pc_query<<<cdiv(nq, 128), 128, 0, s>>>(q, nq, order, hdr, dist, idx);
     LB2_POST_LAUNCH(h, "k_pc_query");
@@ -417,7 +428,11 @@ __device__ __forceinline__ nv3 fe_evec1(const double* A, nv3 e0, double ev1) {
 }
 
 // FastEigen3x3 of the covariance C = {c00, c01, c02, c11, c12, c22}: eigenvector of the smallest eigenvalue, or 0 when max C == 0
+// or when an entry is NaN or infinite (the one-pass sums overflowed: the solver's NaN comparisons would pick an arbitrary branch)
 __device__ __forceinline__ nv3 fast_eigen3x3(const double* C) {
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+        if (!isfinite(C[i])) return {0.0, 0.0, 0.0};
     double mc = C[0];
 #pragma unroll
     for (int i = 1; i < 6; ++i) mc = C[i] > mc ? C[i] : mc;

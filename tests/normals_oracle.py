@@ -7,7 +7,9 @@ open3d install is not pinned (open3d is not a dependency of this project; see DE
   covariance   open3d's one-pass cumulants (ComputeCovariance): sums of x, y, z, xx, xy, xz, yy, yz, zz in neighbour order,
                divided by the count, C = E[ppᵀ] − E[p]E[p]ᵀ; the identity when fewer than 3 neighbours
   normal       FastEigen3x3 (Geometric Tools' robust symmetric 3×3 eigensolver) for the smallest eigenvalue's eigenvector, a zero
-               result replaced by (0, 0, 1), no orientation
+               result replaced by (0, 0, 1), no orientation.  A covariance with a NaN or infinite entry (the cumulants overflow once
+               a neighbourhood's coordinates pass ~1e154) also gives (0, 0, 1): with NaN operands the solver's comparisons pick
+               branches that depend on how each maximum treats NaN, which neither open3d nor Eigen states
 
 Every expression is evaluated in the order the C++ writes it (left to right), one rounding per operation.  The order of the three-term
 dot products inside ComputeEigenvector0 is taken as ((x0·x0 + x1·x1) + x2·x2); Eigen's own reduction order is not pinned either.
@@ -169,7 +171,7 @@ def fast_eigen3x3(cov):
     diag = {"half_det": np.zeros(n), "cross_ratio": np.full(n, np.inf), "evec1_ratio": np.full(n, np.inf)}
     with np.errstate(all="ignore"):
         max_coeff = cov.reshape(n, 9).max(1)
-        live = max_coeff != 0
+        live = (max_coeff != 0) & np.isfinite(cov).all((1, 2))           # a NaN or infinite entry gives the zero vector too
         A = cov / np.where(live, max_coeff, 1.0)[:, None, None]
         a00, a01, a02, a11, a12, a22 = A[:, 0, 0], A[:, 0, 1], A[:, 0, 2], A[:, 1, 1], A[:, 1, 2], A[:, 2, 2]
         norm = (a01 * a01 + a02 * a02) + a12 * a12
