@@ -705,6 +705,50 @@ int lb2_render_splat(void* h, void* stream, const double* pts, int64_t n, const 
 int lb2_render_shade(void* h, void* stream, const uint64_t* keys, const double* pts, const double* normals, const double* colors,
                      double z_lo, double z_hi, const lb2_render_camera* cam, uint8_t* rgb);
 
+/* ---- uniform surface sampling of triangle meshes (mesh.cu, lidiff_b200/mesh.py) — open3d 0.17's
+ * TriangleMesh::SamplePointsUniformly under libstdc++, which lidiff/utils/metrics.py:37 (Metrics3D.convert_to_pcd) calls with
+ * 1 000 000 points.  Every fp64 operation below is rounded on its own (no FMA contraction) so that a sequential host evaluation
+ * (tests/mesh_reference.py) gives the same bits.  Deterministic; no float atomics.
+ *
+ * Inputs: verts fp64 (n_verts, 3), tris int32 (n_tris, 3), N = n_points.
+ *   area_t = 0.5 |x × y| with x = p0 - p1, y = p0 - p2 (p_k = verts[tris[t][k]]), a × b as in lb2_render_*, and
+ *     |c| = sqrt((c0 c0 + c1 c1) + c2 c2);
+ *   S = area_0 + area_1 + ... left to right (surface_area += area);
+ *   cdf_0 = area_0 / S, cdf_t = area_t / S + cdf_{t-1}: a sequential chain (the quotients are independent, the adds are not);
+ *   n_t = round(cdf_t N), half away from zero; triangle t owns the points [n_{t-1}, n_t) (n_{-1} = 0), so point i lies on the
+ *     first t with n_t > i.
+ * Random numbers: point i reads words[4i .. 4i+3] (one uint4; words from lb2_mt19937_words, so a call consumes exactly 4N words of
+ * the stream): r1 from (words[4i], words[4i+1]), r2 from (words[4i+2], words[4i+3]), each libstdc++'s
+ * generate_canonical<double, 53> of std::mt19937 (uniform_real_distribution<double>(0, 1)):
+ *   r = RN(w_lo + w_hi 2^32) 2^-64, and r = nextafter(1, 0) when r >= 1.
+ * The point: s = sqrt(r1), a = 1 - s, b = s (1 - r2), c = s r2; per axis p = (a v0 + b v1) + c v2.
+ *
+ * lb2_mesh_sample_prepare: the areas (area: device fp64[n_tris]), S and the n_t (kept in scratch) and *d_info (device).  Bad input
+ * found on the device is reported in d_info->status, never by a fault:
+ *   LB2_MESH_BAD_INDEX     a vertex index outside [0, n_verts) (that triangle's area is 0);
+ *   LB2_MESH_NON_FINITE    a triangle uses a vertex with a NaN / inf coordinate;
+ *   LB2_MESH_BAD_AREA      S is 0, or not finite (n_t are then not computed);
+ *   LB2_MESH_BAD_COUNT     the last n_t is not N (cannot happen while n_tris N < 2^51: the chain's rounding stays below 1/2).
+ * A caller reads *d_info once and calls lb2_mesh_sample_points only when status == 0.  n_points in [1, 2^53), n_tris >= 1,
+ * n_verts >= 1.  scratch >= lb2_mesh_sample_scratch_bytes(n_tris), 16-byte aligned.
+ * lb2_mesh_sample_points: out (device fp64 (n_points, 3)) from the n_t of the prepare call on the same verts / tris / n_points / scratch;
+ * words: device uint32[4 n_points], 16-byte aligned. */
+#define LB2_MESH_BAD_INDEX   1
+#define LB2_MESH_NON_FINITE  2
+#define LB2_MESH_BAD_AREA    4
+#define LB2_MESH_BAD_COUNT   8
+typedef struct {
+    double  surface_area;   /* S */
+    int64_t last_count;     /* n_{n_tris - 1} (0 when S is bad) */
+    int32_t status;         /* LB2_MESH_* bits */
+    int32_t pad;
+} lb2_mesh_info;
+size_t lb2_mesh_sample_scratch_bytes(int64_t n_tris);
+int lb2_mesh_sample_prepare(void* h, void* stream, const double* verts, int64_t n_verts, const int32_t* tris, int64_t n_tris,
+                            int64_t n_points, double* area, lb2_mesh_info* d_info, void* scratch);
+int lb2_mesh_sample_points(void* h, void* stream, const double* verts, const int32_t* tris, int64_t n_tris, const void* scratch,
+                           const uint32_t* words, int64_t n_points, double* out);
+
 #ifdef __cplusplus
 }
 #endif

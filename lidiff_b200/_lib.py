@@ -79,6 +79,7 @@ EXPORTS = [
     "lb2_sync_bn_backward_max", "lb2_sync_bn_backward_sum", "lb2_sync_bn_backward_apply",
     "lb2_mt19937_words", "lb2_legacy_gauss_scratch_bytes", "lb2_legacy_gauss", "lb2_randperm_scratch_bytes", "lb2_randperm",
     "lb2_render_splat", "lb2_render_shade",
+    "lb2_mesh_sample_scratch_bytes", "lb2_mesh_sample_prepare", "lb2_mesh_sample_points",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -100,6 +101,13 @@ RANDPERM_MAX_N = 214748364          # LB2_RANDPERM_MAX_N = UINT32_MAX // 20
 class RenderCamera(C.Structure):
     _fields_ = [("lookat", C.c_double * 3), ("front", C.c_double * 3), ("up", C.c_double * 3), ("distance", C.c_double),
                 ("focal", C.c_double), ("width", C.c_int32), ("height", C.c_int32)]
+
+
+MESH_BAD_INDEX, MESH_NON_FINITE, MESH_BAD_AREA, MESH_BAD_COUNT = 1, 2, 4, 8      # lb2_mesh_info.status bits
+
+
+class MeshInfo(C.Structure):
+    _fields_ = [("surface_area", C.c_double), ("last_count", C.c_int64), ("status", C.c_int32), ("pad", C.c_int32)]
 
 
 class Segment(C.Structure):
@@ -233,6 +241,10 @@ class Lib:
         d.lb2_randperm.argtypes = [vp, vp, vp, i64, vp, vp, vp]
         d.lb2_render_splat.argtypes = [vp, vp, vp, i64, C.POINTER(RenderCamera), f64, vp]
         d.lb2_render_shade.argtypes = [vp, vp, vp, vp, vp, vp, f64, f64, C.POINTER(RenderCamera), vp]
+        d.lb2_mesh_sample_scratch_bytes.argtypes = [i64]
+        d.lb2_mesh_sample_scratch_bytes.restype = C.c_size_t
+        d.lb2_mesh_sample_prepare.argtypes = [vp, vp, vp, i64, vp, i64, i64, vp, vp, vp]
+        d.lb2_mesh_sample_points.argtypes = [vp, vp, vp, vp, i64, vp, vp, i64, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -648,6 +660,21 @@ class Handle:
         """rgb (uint8 (height, width, 3)) from the keys: white background, colours or jet of z, the headlight of the normals"""
         self._check(self.dll.lb2_render_shade(self.hp, self._stream(), _ptr(keys), _ptr(pts), _ptr(normals), _ptr(colors), float(z_lo),
                                               float(z_hi), C.byref(cam), _ptr(rgb)), "lb2_render_shade")
+
+    # -- uniform surface sampling of triangle meshes (lidiff_b200.mesh) -----------------------------------------------------------
+    def mesh_sample_scratch(self, n_tris: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_mesh_sample_scratch_bytes(int(n_tris)))
+
+    def mesh_sample_prepare(self, verts, tris, n_points, area, info, scratch):
+        """area (fp64 (n_tris,)), S and the status into `info` (a device byte tensor of sizeof(MeshInfo)), the points' triangle
+        bounds n_t into `scratch`, for the fp64 (n_verts, 3) `verts` and int32 (n_tris, 3) `tris`"""
+        self._check(self.dll.lb2_mesh_sample_prepare(self.hp, self._stream(), _ptr(verts), int(verts.shape[0]), _ptr(tris), int(tris.shape[0]),
+                                                     int(n_points), _ptr(area), _ptr(info), _ptr(scratch)), "lb2_mesh_sample_prepare")
+
+    def mesh_sample_points(self, verts, tris, scratch, words, n_points, out):
+        """out (fp64 (n_points, 3)) from a clean mesh_sample_prepare and the 4 n_points MT19937 words `words`"""
+        self._check(self.dll.lb2_mesh_sample_points(self.hp, self._stream(), _ptr(verts), _ptr(tris), int(tris.shape[0]), _ptr(scratch),
+                                                    _ptr(words), int(n_points), _ptr(out)), "lb2_mesh_sample_points")
 
 
 _LIB = None

@@ -7,7 +7,7 @@ mkdir -p "$out"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v)
 objs=()
-for f in coords spconv_ffma spconv_tc spconv_wgrad spconv_scatter dense metrics gate_grad sync_bn maps samples rng render api; do
+for f in coords spconv_ffma spconv_tc spconv_wgrad spconv_scatter dense metrics gate_grad sync_bn maps samples rng render mesh api; do
   src="$here/$f.cu"; obj="$out/$f.o"
   # this script is a dependency too: a change of FLAGS (e.g. the target architecture) rebuilds every object
   if [ ! -f "$obj" ] || [ "$src" -nt "$obj" ] || [ "$here/common.cuh" -nt "$obj" ] || [ "$here/tc_common.cuh" -nt "$obj" ] || [ "$here/../../include/lidiff_b200.h" -nt "$obj" ] || [ "$here/build.sh" -nt "$obj" ]; then

@@ -12,6 +12,9 @@ classes, methods and semantics, computed by the lidiff_b200 CUDA library:
 `evaluate_scan(gt, pred)` computes each direction's distances once and the occupancy once per voxel size and returns a
 `ScanRecord`; the accumulators consume records with `add`, and their `update(gt, pred)` evaluates what they need.  Points may be
 numpy arrays, torch tensors on any device, or open3d-shim PointClouds.  There is no CPU fallback.
+
+`Metrics3D` (the reference's base class of PrecisionRecall) turns a prediction into a point cloud; a triangle mesh is sampled with
+open3d's `sample_points_uniformly(1000000)`, restated bit for bit on the GPU by lidiff_b200.mesh.
 """
 from __future__ import annotations
 
@@ -28,6 +31,8 @@ MAX_RANGE = 50.0                        # histogram range [-MAX_RANGE, MAX_RANGE
 JSD_VOXEL = 0.5                         # histogram_metrics.py:48-49
 VOXEL_SIZES = (0.5, 0.2, 0.1)           # CompletionIoU default
 PR_ARGS = (0.05, 0.1, 100)              # PrecisionRecall(0.05, 2 * 0.05, 100) of eval_path.py
+MESHTYPE, TETRATYPE, PCDTYPE = 6, 10, 1  # open3d GeometryType values (metrics.py:5-7)
+MESH_SAMPLES = 1000000                  # points sampled from a mesh prediction (metrics.py:37)
 
 
 def _xyz(x) -> torch.Tensor | np.ndarray:
@@ -215,7 +220,46 @@ class ChamferDistance:
         return d.mean(), d.std()
 
 
-class PrecisionRecall:
+class Metrics3D:
+    """metrics.py:9-59: whether a prediction is empty, and the prediction as a point cloud.  A geometry is anything with
+    get_geometry_type() (the open3d shim's classes, under either import name); a triangle mesh (type 6) or tetra mesh (10) is
+    converted with its sample_points_uniformly(1000000), which draws from the global stream of open3d.utility.random.  Other
+    types raise TypeError where the reference asserts."""
+
+    def prediction_is_empty(self, geom):
+        if hasattr(geom, "get_geometry_type"):
+            geom_type = geom.get_geometry_type().value
+            if geom_type in (MESHTYPE, TETRATYPE):
+                return self.is_empty(len(geom.vertices)) or self.is_empty(len(geom.triangles))
+            if geom_type == PCDTYPE:
+                return self.is_empty(len(geom.points))
+            raise TypeError(f"{geom.get_geometry_type()} geometry not supported")
+        if isinstance(geom, (np.ndarray, torch.Tensor)):
+            return self.is_empty(len(geom[:, :3]))
+        raise TypeError(f"{type(geom)} type not supported")
+
+    @staticmethod
+    def convert_to_pcd(geom):
+        from .shims.open3d.geometry import PointCloud
+        if hasattr(geom, "get_geometry_type"):
+            geom_type = geom.get_geometry_type().value
+            if geom_type in (MESHTYPE, TETRATYPE):
+                return geom.sample_points_uniformly(MESH_SAMPLES)
+            if geom_type == PCDTYPE:
+                return geom
+            raise TypeError(f"{geom.get_geometry_type()} geometry not supported")
+        if isinstance(geom, torch.Tensor):
+            geom = geom.detach().cpu().numpy()
+        if isinstance(geom, np.ndarray):
+            return PointCloud(geom[:, :3])
+        raise TypeError(f"{type(geom)} type not supported")
+
+    @staticmethod
+    def is_empty(length):
+        return not length
+
+
+class PrecisionRecall(Metrics3D):
     """precision (share of predicted points closer than t to the gt) and recall (share of gt points closer than t to the
     prediction) in percent at np.linspace(min_t, max_t, num) thresholds, F-score 0 when either is 0; averaged over scans"""
 

@@ -1,6 +1,6 @@
 import numpy as np
 
-from .utility import Vector3dVector
+from .utility import Vector3dVector, Vector3iVector
 
 
 class KDTreeSearchParamKNN:
@@ -22,6 +22,7 @@ class GeometryType:
         def __init__(self, v):
             self.value = v
     Unspecified, PointCloud, VoxelGrid = _T(0), _T(1), _T(2)
+    TriangleMesh = _T(6)
 
 
 def _knn(query, ref, k):
@@ -196,3 +197,44 @@ class PointCloud(Geometry):
                 out[a:a + 65536] = torch.linalg.eigh(cov.double())[1][:, :, 0].float()   # eigenvector of the smallest eigenvalue
         self._normals = Vector3dVector(out.cpu().numpy())
         return True
+
+
+class TriangleMesh(Geometry):
+    """vertices (Vector3dVector) and triangles (Vector3iVector) — what lidiff/utils/metrics.py's Metrics3D reads from a mesh
+    prediction.  `sample_points_uniformly` is open3d 0.17's, bit for bit, on the GPU (lidiff_b200.mesh) and draws from the global
+    stream of `utility.random`.  Vertex normals and colours are not kept and not carried into the sampled cloud: the metrics never
+    read them.  No CPU fallback."""
+
+    def __init__(self, vertices=None, triangles=None):
+        self._vertices = Vector3dVector(vertices if vertices is not None else ())
+        self._triangles = Vector3iVector(triangles if triangles is not None else ())
+
+    vertices = property(lambda s: s._vertices, lambda s, v: setattr(s, "_vertices", Vector3dVector(v)))
+    triangles = property(lambda s: s._triangles, lambda s, v: setattr(s, "_triangles", Vector3iVector(v)))
+
+    def __repr__(self):
+        return f"TriangleMesh with {len(self._vertices)} points and {len(self._triangles)} triangles."
+
+    def has_vertices(self):
+        return len(self._vertices) > 0
+
+    def has_triangles(self):
+        return len(self._vertices) > 0 and len(self._triangles) > 0
+
+    def get_geometry_type(self):
+        return GeometryType.TriangleMesh
+
+    def get_surface_area(self):
+        """the sum of the triangle areas, left to right, as open3d adds them (lidiff_b200.mesh.surface_area)"""
+        from lidiff_b200.mesh import surface_area
+        return surface_area(np.asarray(self._vertices), np.asarray(self._triangles))
+
+    def sample_points_uniformly(self, number_of_points=100, use_triangle_normal=False):
+        """a PointCloud of `number_of_points` points drawn uniformly from the surface (open3d's SamplePointsUniformly); the global
+        stream of utility.random advances by 4 number_of_points words.  Raises ValueError for number_of_points <= 0, a mesh without
+        triangles, a vertex index out of range, a NaN / inf vertex of a triangle or a zero surface area."""
+        if use_triangle_normal:
+            raise NotImplementedError("open3d shim: sample_points_uniformly carries no normals (use_triangle_normal=True)")
+        from lidiff_b200.mesh import STREAM
+        pts = STREAM.sample_points_uniformly(np.asarray(self._vertices), np.asarray(self._triangles), number_of_points)
+        return PointCloud(pts.cpu().numpy())

@@ -8,7 +8,9 @@ cd_mean, cd_std, pr, re, f1) next to --path, with every metric computed on the G
 
 Two modes: with -d / -r (or --random-weights) every scan is completed with lidiff_b200.pipeline.DiffCompletion and the refined
 cloud is scored (--cloud diff scores the diffusion-only cloud); without them the `<stem>.ply` files in --path are scored, as
-lidiff_b200.tools.diff_completion_pipeline writes them.  Under torchrun scan b runs on rank b mod R; rank 0 folds the per-scan
+lidiff_b200.tools.diff_completion_pipeline writes them.  With --mesh those files are triangle meshes (io.read_triangle_mesh), each
+turned into 1 000 000 points by Metrics3D.convert_to_pcd (open3d's sample_points_uniformly, on the GPU) from the std::mt19937 seeded
+with --seed plus the scan's index in the sorted listing, so the samples do not depend on the number of ranks.  Under torchrun scan b runs on rank b mod R; rank 0 folds the per-scan
 records in scan order, so the results do not depend on the number of ranks.  --batch-size B completes a rank's scans B at a
 time (DiffCompletion.complete_scans); res_log.yaml has the same layout as with B = 1.
 """
@@ -45,12 +47,25 @@ def scan_completion(data: str, scan_name: str, path: str, pipe, max_range: float
     return scan_completions(data, [scan_name], path, pipe, max_range, cloud)[0]
 
 
-def scan_completions(data: str, scan_names: list, path: str, pipe, max_range: float, cloud: str, batched: bool = False):
+def read_mesh_prediction(path: str, seed: int) -> np.ndarray:
+    """the points Metrics3D.convert_to_pcd samples from the triangle mesh at `path`, with the global stream seeded with `seed`"""
+    from ..mesh import STREAM
+    from ..shims.open3d.io import read_triangle_mesh
+    STREAM.seed(seed)
+    return np.asarray(M.Metrics3D.convert_to_pcd(read_triangle_mesh(path)).points)
+
+
+def scan_completions(data: str, scan_names: list, path: str, pipe, max_range: float, cloud: str, batched: bool = False,
+                     mesh_seeds: list | None = None):
     """[(prediction, the scan's points within max_range)] of a group of scans; batched: completed by complete_scans (one
-    trajectory per scan, a group shorter than the others starts fresh), else one by one by complete_scan"""
+    trajectory per scan, a group shorter than the others starts fresh), else one by one by complete_scan; mesh_seeds (files
+    only): the predictions are triangle meshes, sampled with these seeds"""
     points = [np.fromfile(os.path.join(data, "velodyne", s), dtype=np.float32).reshape(-1, 4) for s in scan_names]
     curs = [p[np.sqrt(np.sum(p[:, :3] ** 2, axis=-1)) < max_range, :3] for p in points]
-    if pipe is None:
+    if pipe is None and mesh_seeds is not None:
+        preds = [read_mesh_prediction(os.path.join(path, f"{s.split('.')[0]}.ply"), seed) for s, seed in zip(scan_names, mesh_seeds)]
+        preds = [p[np.sqrt(np.sum(p ** 2, axis=-1)) < max_range] for p in preds]
+    elif pipe is None:
         preds = [read_ply_xyz(os.path.join(path, f"{s.split('.')[0]}.ply")) for s in scan_names]
         preds = [p[np.sqrt(np.sum(p ** 2, axis=-1)) < max_range] for p in preds]
     else:
@@ -59,15 +74,18 @@ def scan_completions(data: str, scan_names: list, path: str, pipe, max_range: fl
     return list(zip(preds, curs))
 
 
-def score_scans(data: str, path: str, pipe, max_range: float, cloud: str, device, rank: int = 0, world: int = 1, batch: int = 1):
-    """(number of scans, {scan index: record as rows}) for the scans of this rank, completed `batch` at a time"""
+def score_scans(data: str, path: str, pipe, max_range: float, cloud: str, device, rank: int = 0, world: int = 1, batch: int = 1,
+                mesh_seed: int | None = None):
+    """(number of scans, {scan index: record as rows}) for the scans of this rank, completed `batch` at a time; mesh_seed: the
+    predictions are triangle meshes, scan b sampled with seed mesh_seed + b"""
     poses = load_poses(os.path.join(data, "calib.txt"), os.path.join(data, "poses.txt"))
     seq_map = np.load(os.path.join(data, "map_clean.npy"))
     scans = natural_sorted(os.listdir(os.path.join(data, "velodyne")))
     n = min(len(poses), len(scans))
     local = {}
     for group in batches_of_rank(n, world, rank, batch):
-        for b, (pred, cur) in zip(group, scan_completions(data, [scans[b] for b in group], path, pipe, max_range, cloud, batch > 1)):
+        seeds = None if mesh_seed is None else [mesh_seed + b for b in group]
+        for b, (pred, cur) in zip(group, scan_completions(data, [scans[b] for b in group], path, pipe, max_range, cloud, batch > 1, seeds)):
             gt = ground_truth(poses[b], cur, seq_map, max_range)
             local[b] = M.record_to_rows(M.evaluate_scan(gt, pred, device=device))
     return n, local
@@ -130,7 +148,11 @@ def log_path(path: str) -> str:
 @click.option("--data", type=str, default=PATH_DATA, help="sequence directory: velodyne/*.bin, calib.txt, poses.txt, map_clean.npy")
 @click.option("--cloud", type=click.Choice(["refine", "diff"]), default="refine", help="which completed cloud to score")
 @click.option("--batch-size", type=click.IntRange(min=1), default=1, help="scans completed together per denoising loop (default: 1)")
-def main(path, voxel_size, max_range, denoising_steps, cond_weight, diff, refine, random_weights, data, cloud, batch_size):
+@click.option("--mesh", is_flag=True, help="the .ply predictions are triangle meshes: score 1 000 000 points sampled from each surface")
+@click.option("--seed", type=click.IntRange(min=0), default=0, help="with --mesh: scan b is sampled with std::mt19937(seed + b)")
+def main(path, voxel_size, max_range, denoising_steps, cond_weight, diff, refine, random_weights, data, cloud, batch_size, mesh, seed):
+    if mesh and (random_weights or diff is not None or refine is not None):
+        raise click.UsageError("--mesh scores mesh files; it cannot be combined with -d / -r / --random-weights")
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)))
     torch.cuda.set_device(device)
@@ -146,7 +168,7 @@ def main(path, voxel_size, max_range, denoising_steps, cond_weight, diff, refine
     elif diff is not None or refine is not None:
         from ..pipeline import DiffCompletion
         pipe = DiffCompletion(diff, refine, denoising_steps, cond_weight, device=device)
-    n, local = score_scans(data, path, pipe, max_range, cloud, device, rank, world, batch_size)
+    n, local = score_scans(data, path, pipe, max_range, cloud, device, rank, world, batch_size, seed if mesh else None)
     gathered = gather_scans(local, n, device)
     if rank == 0:
         res = fold({b: M.record_from_rows(rows) for b, rows in gathered.items()})
