@@ -749,6 +749,55 @@ int lb2_mesh_sample_prepare(void* h, void* stream, const double* verts, int64_t 
 int lb2_mesh_sample_points(void* h, void* stream, const double* verts, const int32_t* tris, int64_t n_tris, const void* scratch,
                            const uint32_t* words, int64_t n_points, double* out);
 
+/* ---- SemanticKITTI scene-completion (SSC) voxel grids (ssc.cu, lidiff_b200/ssc.py) — the format of the semantic-kitti-api
+ * development kit (auxiliary/io_data.py, generate_sequential.py), restated; lidiff_b200/ssc.py holds the same constants.
+ *
+ * The grid is (256, 256, 32) voxels of 0.2 m in C order, v = (i 256 + j) 32 + k, over [min, max) with min = (0, -25.6, -2) and
+ * max = (51.2, 25.6, 4.4), in the scan's frame.
+ *   Packed bits (`.bin`, `.invalid`, 262 144 bytes): voxel v is bit 7 - (v & 7) of byte v >> 3 (MSB first).  On the device a grid
+ *     is LB2_SSC_WORDS uint32 whose little-endian bytes are the file's bytes, so voxel v is bit (v & 31) ^ 7 of word v >> 5.
+ *   Labels (`.label`): LB2_SSC_VOXELS little-endian uint16.  A voxel is occupied iff its label is neither 0 (empty) nor 255 (ignore).
+ *   Voxel -> point: the centre, min_d + (idx_d + 0.5) 0.2 per axis in fp64 (the product and the sum each rounded).
+ *   Point -> voxel: idx_d = floor((p_d - min_d) / 0.2) per axis in fp64 (difference and quotient each rounded); the point lies in the
+ *     grid iff every idx_d is in [0, dim_d).  A row with a NaN / inf coordinate is dropped and counted, never clamped.
+ *
+ * lb2_ssc_grid_count: G grids (kind LB2_SSC_BITS: uint32[G][LB2_SSC_WORDS]; LB2_SSC_LABELS: uint16[G][LB2_SSC_VOXELS], device) ->
+ *   offsets (device int64[G + 1]): offsets[0] = 0, offsets[g + 1] - offsets[g] = the occupied voxels of grid g; the per-word
+ *   occupancy and in-grid positions stay in scratch (>= lb2_ssc_scratch_bytes(G), 16-byte aligned).  Three launches.
+ * lb2_ssc_grid_points: out (device fp64 (offsets[G], 3)) = the centres of every grid's occupied voxels, grid after grid, each grid's
+ *   in ascending v (np.nonzero's order), from the scratch of a grid_count call on the same G (one launch; no atomics: the same
+ *   bytes on every run).  A caller reads offsets[G] in between to size out.
+ * lb2_ssc_voxelize: G clouds, rows [offsets[g], offsets[g + 1]) of pts (device fp64 (n, 3); offsets device int64[G + 1],
+ *   offsets[G] = n) -> bits (device uint32[G][LB2_SSC_WORDS], cleared first; each point's voxel set by atomicOr) and
+ *   d_info[g] (device, cleared first): the rows dropped as non-finite and as outside the grid.
+ * lb2_ssc_confusion: out (device int64[G][3]) = (TP, FP, FN) of predicted occupancy bits (uint32[G][LB2_SSC_WORDS]) against
+ *   ground-truth labels (uint16[G][LB2_SSC_VOXELS]) over the valid voxels: a voxel is invalid when its label is 255 or its bit of
+ *   `invalid` (uint32[G][LB2_SSC_WORDS], NULL: none) is set.  TP = pred & gt, FP = pred & !gt, FN = !pred & gt, gt = occupied.
+ *   Integer popcounts; the same counts on every run. */
+#define LB2_SSC_DIM_X   256
+#define LB2_SSC_DIM_Y   256
+#define LB2_SSC_DIM_Z   32
+#define LB2_SSC_VOXELS  2097152      /* 256 x 256 x 32 */
+#define LB2_SSC_WORDS   65536        /* LB2_SSC_VOXELS / 32 */
+#define LB2_SSC_VOXEL   0.2
+#define LB2_SSC_MIN_X   0.0
+#define LB2_SSC_MIN_Y   (-25.6)
+#define LB2_SSC_MIN_Z   (-2.0)
+#define LB2_SSC_IGNORE  255
+#define LB2_SSC_BITS    0
+#define LB2_SSC_LABELS  1
+typedef struct {
+    int64_t non_finite;     /* rows with a NaN / inf coordinate */
+    int64_t outside;        /* finite rows outside the grid */
+} lb2_ssc_voxel_info;
+size_t lb2_ssc_scratch_bytes(int64_t n_grids);
+int lb2_ssc_grid_count(void* h, void* stream, const void* grids, int32_t kind, int64_t n_grids, int64_t* offsets, void* scratch);
+int lb2_ssc_grid_points(void* h, void* stream, int64_t n_grids, const int64_t* offsets, const void* scratch, double* out);
+int lb2_ssc_voxelize(void* h, void* stream, const double* pts, const int64_t* offsets, int64_t n_grids, int64_t n_points,
+                     uint32_t* bits, lb2_ssc_voxel_info* d_info);
+int lb2_ssc_confusion(void* h, void* stream, const uint32_t* pred_bits, const uint16_t* gt_labels, const uint32_t* invalid,
+                      int64_t n_grids, int64_t* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -80,6 +80,7 @@ EXPORTS = [
     "lb2_mt19937_words", "lb2_legacy_gauss_scratch_bytes", "lb2_legacy_gauss", "lb2_randperm_scratch_bytes", "lb2_randperm",
     "lb2_render_splat", "lb2_render_shade",
     "lb2_mesh_sample_scratch_bytes", "lb2_mesh_sample_prepare", "lb2_mesh_sample_points",
+    "lb2_ssc_scratch_bytes", "lb2_ssc_grid_count", "lb2_ssc_grid_points", "lb2_ssc_voxelize", "lb2_ssc_confusion",
 ]
 
 RANGE_NONE, RANGE_FP32, RANGE_FP64 = 0, 1, 2
@@ -108,6 +109,13 @@ MESH_BAD_INDEX, MESH_NON_FINITE, MESH_BAD_AREA, MESH_BAD_COUNT = 1, 2, 4, 8     
 
 class MeshInfo(C.Structure):
     _fields_ = [("surface_area", C.c_double), ("last_count", C.c_int64), ("status", C.c_int32), ("pad", C.c_int32)]
+
+
+SSC_BITS, SSC_LABELS = 0, 1        # lb2_ssc_grid_count's kinds
+
+
+class SscVoxelInfo(C.Structure):
+    _fields_ = [("non_finite", C.c_int64), ("outside", C.c_int64)]
 
 
 class Segment(C.Structure):
@@ -245,6 +253,12 @@ class Lib:
         d.lb2_mesh_sample_scratch_bytes.restype = C.c_size_t
         d.lb2_mesh_sample_prepare.argtypes = [vp, vp, vp, i64, vp, i64, i64, vp, vp, vp]
         d.lb2_mesh_sample_points.argtypes = [vp, vp, vp, vp, i64, vp, vp, i64, vp]
+        d.lb2_ssc_scratch_bytes.argtypes = [i64]
+        d.lb2_ssc_scratch_bytes.restype = C.c_size_t
+        d.lb2_ssc_grid_count.argtypes = [vp, vp, vp, i32, i64, vp, vp]
+        d.lb2_ssc_grid_points.argtypes = [vp, vp, i64, vp, vp, vp]
+        d.lb2_ssc_voxelize.argtypes = [vp, vp, vp, vp, i64, i64, vp, vp]
+        d.lb2_ssc_confusion.argtypes = [vp, vp, vp, vp, vp, i64, vp]
         self._handles = {}
         self._lock = threading.Lock()
 
@@ -675,6 +689,32 @@ class Handle:
         """out (fp64 (n_points, 3)) from a clean mesh_sample_prepare and the 4 n_points MT19937 words `words`"""
         self._check(self.dll.lb2_mesh_sample_points(self.hp, self._stream(), _ptr(verts), _ptr(tris), int(tris.shape[0]), _ptr(scratch),
                                                     _ptr(words), int(n_points), _ptr(out)), "lb2_mesh_sample_points")
+
+    # -- SemanticKITTI scene-completion grids (lidiff_b200.ssc) -------------------------------------------------------------------
+    def ssc_scratch(self, n_grids: int) -> torch.Tensor:
+        return self._bytes(self.dll.lb2_ssc_scratch_bytes(int(n_grids)))
+
+    def ssc_grid_count(self, grids, kind, n_grids, offsets, scratch):
+        """offsets (int64 (n_grids + 1,)) <- the running totals of the occupied voxels of the device grids (SSC_BITS: uint32 words,
+        SSC_LABELS: uint16 labels); the per-word occupancy stays in `scratch` for ssc_grid_points"""
+        self._check(self.dll.lb2_ssc_grid_count(self.hp, self._stream(), _ptr(grids), int(kind), int(n_grids), _ptr(offsets),
+                                                _ptr(scratch)), "lb2_ssc_grid_count")
+
+    def ssc_grid_points(self, n_grids, offsets, scratch, out):
+        """out (fp64 (offsets[n_grids], 3)) <- the occupied voxels' centres of a ssc_grid_count call"""
+        self._check(self.dll.lb2_ssc_grid_points(self.hp, self._stream(), int(n_grids), _ptr(offsets), _ptr(scratch), _ptr(out)),
+                    "lb2_ssc_grid_points")
+
+    def ssc_voxelize(self, pts, offsets, n_grids, bits, info):
+        """bits (uint32 as int32 (n_grids, 65536)) <- the packed grids of the fp64 (n, 3) `pts`, cloud g = rows [offsets[g],
+        offsets[g + 1]); info (a device byte tensor of n_grids SscVoxelInfo) <- the dropped rows"""
+        self._check(self.dll.lb2_ssc_voxelize(self.hp, self._stream(), _ptr(pts), _ptr(offsets), int(n_grids), int(pts.shape[0]),
+                                              _ptr(bits), _ptr(info)), "lb2_ssc_voxelize")
+
+    def ssc_confusion(self, pred_bits, gt_labels, invalid, n_grids, out):
+        """out (int64 (n_grids, 3)) <- TP, FP, FN of the packed predictions against the labels, over the valid voxels"""
+        self._check(self.dll.lb2_ssc_confusion(self.hp, self._stream(), _ptr(pred_bits), _ptr(gt_labels), _ptr(invalid), int(n_grids),
+                                               _ptr(out)), "lb2_ssc_confusion")
 
 
 _LIB = None

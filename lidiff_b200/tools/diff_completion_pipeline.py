@@ -5,6 +5,8 @@
 normals as `nx ny nz`, computed on the GPU by lidiff_b200.normals), plus sharding of the scans over the ranks of a torchrun job
 (one process per GPU, scan b on rank b mod R; SURVEY.md 8e).  --batch-size B completes a rank's scans B at a time
 (DiffCompletion.complete_scans: one trajectory per scan, every launch shared); the files written are the same as with B = 1.
+With --ssc each refined cloud is also written as a SemanticKITTI scene-completion grid, `results/<exp>/ssc/<scan>.bin` (the 0.2 m
+256 x 256 x 32 occupancy of lidiff_b200.ssc, voxelized on the GPU), which `eval_path --voxels` and SSC tools read.
 
     torchrun --nproc-per-node 8 -m lidiff_b200.tools.diff_completion_pipeline -d diff.ckpt -r refine.ckpt --path ./Datasets/test
     python -m lidiff_b200.tools.diff_completion_pipeline --random-weights --path ./Datasets/test     # no checkpoints at hand
@@ -19,6 +21,7 @@ import numpy as np
 import torch
 
 from ..normals import estimate_normals
+from .. import ssc as S
 from ..pipeline import DiffCompletion
 from ..sharding import batches_of_rank
 from ..synth import read_ply_xyz
@@ -58,7 +61,8 @@ def write_ply(path: str, pts: np.ndarray, normals: np.ndarray | None = None):
 @click.option("--random-weights", is_flag=True, help="seeded random parameters instead of checkpoints (plumbing / benchmarking)")
 @click.option("--normals", is_flag=True, help="write open3d's estimate_normals() (30 nearest neighbours) as nx ny nz, as the reference does")
 @click.option("--batch-size", type=click.IntRange(min=1), default=1, help="scans completed together per denoising loop (default: 1)")
-def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, normals, batch_size):
+@click.option("--ssc", is_flag=True, help="also write each refined cloud as a SemanticKITTI scene-completion grid, ssc/<scan>.bin")
+def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, normals, batch_size, ssc):
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
     device = torch.device("cuda", local_rank)
@@ -75,6 +79,8 @@ def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, 
         pipe = DiffCompletion(diff, refine, denoising_steps, cond_weight, device=device)
     os.makedirs(f"{out}/{exp_dir}/refine", exist_ok=True)
     os.makedirs(f"{out}/{exp_dir}/diff", exist_ok=True)
+    if ssc:
+        os.makedirs(f"{out}/{exp_dir}/ssc", exist_ok=True)
     files = sorted(os.listdir(path), key=lambda s: [int(t) if t.isdigit() else t for t in __import__("re").split(r"(\d+)", s)])
     for group in batches_of_rank(len(files), world, rank, batch_size):
         names = [files[i] for i in group]
@@ -88,6 +94,8 @@ def main(diff, refine, denoising_steps, cond_weight, path, out, random_weights, 
             for kind, cloud in (("refine", refine_scan), ("diff", diff_scan)):
                 nrm = estimate_normals(cloud, device=device).cpu().numpy() if normals else None
                 write_ply(f"{out}/{exp_dir}/{kind}/{stem}.ply", cloud, nrm)
+            if ssc:
+                S.write_bin(f"{out}/{exp_dir}/ssc/{stem}.bin", S.voxelize(refine_scan, device=device)[0])
     if world > 1:
         import torch.distributed as dist
         dist.barrier()
