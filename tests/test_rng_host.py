@@ -142,21 +142,6 @@ def test_libm_log_is_correctly_rounded_outside_the_band():
     assert (dn < 0.01).sum() > 100                                   # the constructed inputs do reach the band
 
 
-def _crafted_state(words_wanted):
-    """a numpy state at pos 620 whose next four words are `words_wanted` (the key holds their untempered values)"""
-    rs = np.random.RandomState(0)
-    _, key, _, _, _ = rs.get_state(legacy=True)
-    key = key.copy()
-    key[620:624] = rng.untemper(np.asarray(words_wanted, np.uint32))
-    rs.set_state(("MT19937", key, 620, 0, 0.0))
-    return rs
-
-
-def _words_for(d1, d2):
-    """the 4 words whose legacy doubles are the 53-bit integers d1, d2 (x = 2 d 2^-53 - 1)"""
-    return [(d1 >> 26) << 5, (d1 & ((1 << 26) - 1)) << 6, (d2 >> 26) << 5, (d2 & ((1 << 26) - 1)) << 6]
-
-
 @pytest.mark.parametrize("case,d1,d2,accepted", [
     ("r2_zero", 1 << 52, 1 << 52, False),                      # x1 = x2 = 0
     ("x_minus_one", 0, 1 << 52, False),                        # x1 = -1, x2 = 0: r2 = 1
@@ -165,7 +150,7 @@ def _words_for(d1, d2):
     ("largest_r2", 1, 1 << 52, True),                          # x1 = -1 + 2^-52: r2 just below 1
 ])
 def test_crafted_states_reach_the_polar_edges(case, d1, d2, accepted):
-    rs = _crafted_state(_words_for(d1, d2))
+    rs = R.crafted_state(R.words_for(d1, d2))
     _, key, pos, hg, g = rs.get_state(legacy=True)
     words, _, _ = R.mt_words(key, pos, 4)
     x1, x2, r2, acc = R.attempts(words)
